@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/sec across the ES population (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- env-steps/sec across the ES population (BASELINE.json metric) on N H100s of one node.
 
 Workload (BASELINE.json configs[1], SURVEY.md 8d config 2): Frostbite-shaped ES generation, population 1000
 (n = 500 antithetic pairs), LargeModel conv policy (P = 4,052,658, 18 actions), 256 resident env slots per GPU (--slots), synthetic
@@ -14,8 +14,11 @@ One "step" = one GENERATION: rollouts of this rank's shard of the population for
   --impl reference   the reference worker/master loop restated on the CPU (oracle/cpu_worker.py) on all host cores.
 
 Timing: >= 3 warm-up steps; device timing with CUDA events bracketed by barrier + synchronize, max over ranks.
-Every tick streams >= 1 GB of noise slices (>> 126 MB L2) so no input survives in L2 between timed iterations
+Every tick streams >= 1 GB of noise slices (>> 50 MB L2) so no input survives in L2 between timed iterations
 (config.l2: "inputs larger than L2").
+The inputs (weights, observations, rewards, noise indices) are seeded, so runs with the same arguments see the same inputs;
+--dump-outputs DIR writes what the last timed generation computed (updated theta, gradient, returns, last tick's logits and
+actions) as .npy files, for comparing two builds output for output.
 """
 from __future__ import annotations
 
@@ -45,7 +48,8 @@ def parse():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference", "cpu-sample", "gpu-ref-proxy"])
+    ap.add_argument("--impl", default="gpu", choices=["gpu", "b200", "reference", "cpu-sample", "gpu-ref-proxy"],
+                    help="gpu: this library on the GPU (b200: older name of the same arm)")
     ap.add_argument("--workload", default="es", choices=["es", "mlp", "ga", "nsr"],
                     help="es = BASELINE.json configs[1] (the contract's default line); mlp / ga / nsr = configs[4] / [2] / [3] "
                          "(bench_workloads.py), same JSON contract")
@@ -56,7 +60,12 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-sample-steps", type=int, default=40, help="env steps per episode in the CPU sample")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed generation's outputs to DIR/<name>.npy (es workload)")
+    a = ap.parse_args()
+    if a.dump_outputs and (a.impl not in ("gpu", "b200") or a.workload != "es"):
+        ap.error("--dump-outputs is implemented for the default arm only (--impl gpu --workload es)")
+    return a
 
 
 def load_peaks():
@@ -64,7 +73,7 @@ def load_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (700 W)"
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -131,7 +140,7 @@ def exp_dict(args):
     }
 
 
-def run_b200(args):
+def run_gpu(args):
     import torch
     import torch.distributed as dist
     from dne import _ffi as F, nets, shard
@@ -168,7 +177,7 @@ def run_b200(args):
     # of 128 pairs per generation at pop 1000): every kernel runs alone, so the per-launch GEMV timing in `roofline` and
     # the ncu launch list describe the same schedule.  `--slots 1024` gives every antithetic pair a resident slot pair
     # (one wave per generation) split over 4 tables on 4 streams, whose conv chains overlap each other's HBM-bound
-    # GEMV: r01 624K vs 527-540K env-steps/s (profiles/r01_bench_n1_1000slots.json; tools/sweep_overlap.py).
+    # GEMV (tools/sweep_overlap.py).
     # DNE_BENCH_STREAMS overrides NS; DNE_BENCH_PHASED=1 adds the phase-event hand-off (dne_set_phase_events).
     pairs_local = hi - lo
     slots = max(2, min(args.slots, 2 * pairs_local))
@@ -183,8 +192,10 @@ def run_b200(args):
     for e in phase_ev:
         e.record()                                               # materialise the handles
     R = 4                                                        # observation pool blocks, rotated every tick
-    pool = torch.randint(0, 256, (R, slots, 84, 84, 4), dtype=torch.uint8, device=dev)
-    rew_pool = (torch.rand(64, slots, device=dev) < 0.05).float() * 10.0
+    gen = torch.Generator(device=dev)
+    gen.manual_seed(1234 + rank)                                 # same inputs on every run with the same arguments
+    pool = torch.randint(0, 256, (R, slots, 84, 84, 4), dtype=torch.uint8, device=dev, generator=gen)
+    rew_pool = (torch.rand(64, slots, device=dev, generator=gen) < 0.05).float() * 10.0
     ret_acc = torch.zeros(slots, device=dev)
     idx_stream = np.random.RandomState(1)
     tally = {"launches": 0, "pairs": 0}
@@ -201,8 +212,8 @@ def run_b200(args):
     KERNELS_PER_TICK = 6          # conv1-3, theta GEMM, noise GEMV, combine+head (LargeModel, default options)
     # Tick launch.  Default: kernel by kernel on one stream, the six kernels AND consecutive ticks chained by programmatic
     # dependent launch (DESIGN 3.1; dne_set_option("chain_ticks", 1): with device-resident observations the stream's previous
-    # kernel of a tick's first convolution is the previous tick's head) -- interleaved A/B (tools/ab_tick.py): 2-5 us per tick
-    # faster than one CUDA graph per tick, whose launch boundary is a full dependency.  DNE_BENCH_GRAPH=1 replays graphs.
+    # kernel of a tick's first convolution is the previous tick's head), so that no tick boundary is a full dependency as a
+    # CUDA graph's launch boundary is (tools/ab_tick.py compares the two).  DNE_BENCH_GRAPH=1 replays graphs.
     USE_GRAPH = os.environ.get("DNE_BENCH_GRAPH", "0") == "1"
     CHAIN = (not USE_GRAPH) and os.environ.get("DNE_BENCH_CHAIN", "1") == "1"
     if NS >= 2 and PHASED:
@@ -223,6 +234,7 @@ def run_b200(args):
             bd.append((tag, time.perf_counter()))
 
     rollout_ev = []              # (start, end) CUDA events around the rollout part of every generation (this rank's own work)
+    last = {}                    # what the latest generation computed (--dump-outputs)
 
     def generation_value():
         mark("start")
@@ -310,6 +322,7 @@ def run_b200(args):
         g = upd.gradient(proc[lo:hi].contiguous(), torch.from_numpy(my).to(dev), denom=2 * n_pairs)
         shard.all_reduce_sum_(g)
         upd.step(L2)
+        last.update(returns=allret, grad=g)
         mark("update")
         if BREAKDOWN:
             t0 = bd[0][1]
@@ -382,13 +395,7 @@ def run_b200(args):
     survey_bytes = 2 * pairs_per_launch * (4.0 * P + 84 * 84 * 4 + 4)
     avg_ms = tot_ms / max(n_timed, 1)
     achieved = alg_bytes / (avg_ms * 1e-3) / 1e9 if n_timed else None
-    traffic = None
-    try:      # DRAM bytes of the same kernel from the committed ncu --set full capture, scaled to this run's pairs/launch
-        with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as f:
-            tj = json.load(f)["gemv_bulk_kernel"]
-        traffic = tj["dram_bytes_per_launch"] * pairs_per_launch / tj["pairs_per_launch"]
-    except Exception:
-        pass
+    traffic = None               # measured DRAM bytes per launch: needs a hardware-counter profile, not taken here
     roofline = {"bound": "hbm",
                 "kernel": "gemv_bulk_kernel<2> (fc 7744x512 noise GEMV: cp.async.bulk ring, slice shared by the +/- pair)",
                 "achieved": achieved, "peak": peaks["hbm_gbs"], "peak_source": peak_src, "unit": "GB/s",
@@ -403,6 +410,11 @@ def run_b200(args):
                 "note": "algorithmic bytes = one fc noise slice per antithetic PAIR (read once for both members); "
                         "survey_bytes = SURVEY 8d figure (4P + obs + action per env-step, every member its own slice). "
                         "~5% of the slice bytes hit in L2 (random 16 MB slices of a 1 GB table overlap), hence frac > 1."}
+
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {
+            "theta": upd.theta, "grad": last["grad"], "returns": last["returns"],
+            "logits": torch.cat([sf.logits for sf in sfs]), "actions": torch.cat([sf.actions for sf in sfs])})
 
     # ------------------------------------------------------------------ output check of the benchmarked kernels
     parity = parity_check(L, ctx, net, sfs[0], upd.theta, obs_ptr[0][0], pool[0][:part], part)
@@ -431,6 +443,8 @@ def run_b200(args):
                 shard.barrier()
                 torch.cuda.synchronize()
                 marks[it] = time.perf_counter()
+        if args.warmup == 0:         # run_master numbers its iterations from 1: without warm-up the window opens here
+            on_it(0, None, None)
         ES.run_master(None, None, exp_dict(args), max_iterations=args.warmup + args.steps, n_slots=slots_e2e,
                       env=env, noise=noise, seed=0, on_iteration=on_it)
         dt = marks[args.warmup + args.steps] - marks[args.warmup]
@@ -474,9 +488,19 @@ def run_b200(args):
 
 
 # ---------------------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy for every array: float tensors as float32, integer ones (actions) converted to float32 too."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().to("cpu", torch.float32).numpy() if isinstance(t, torch.Tensor) else np.asarray(t, np.float32)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
+# ---------------------------------------------------------------------------------------------------------------
 def parity_check(L, ctx, net, sf, theta, obs_p, obs, n_slots):
     """After the timed region: one tick of the benchmarked slot table (whatever indices / active mask the last wave
-    left in it) through the benchmarked kernels (tcgen05 convolutions + TMA bulk-copy GEMV) and through the plain fp32
+    left in it) through the benchmarked kernels (wgmma convolutions + TMA bulk-copy GEMV) and through the plain fp32
     SIMT kernels (dne_set_option conv_tc = 0, gemv_bulk = 0; same C ABI, no oracle involved): logits within twice the
     forward bound of tests/test_gpu_parity.py on every active slot, identical actions wherever the top-2 gap decides."""
     import ctypes as C
@@ -635,4 +659,4 @@ if __name__ == "__main__":
         import bench_workloads
         bench_workloads.run(a, _emit, ClockSampler, load_peaks)
     else:
-        run_b200(a)
+        run_gpu(a)

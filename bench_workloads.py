@@ -233,6 +233,8 @@ def run(args, emit, ClockSampler, load_peaks):
                 torch.cuda.synchronize()
                 marks[it] = time.perf_counter()
         kw = dict(max_iterations=args.warmup + args.steps, n_slots=s4, noise=noise, seed=0, on_iteration=on_it)
+        if args.warmup == 0:         # run_master numbers its iterations from 1: without warm-up the window opens here
+            on_it(0, None, None)
         if wl == "mlp":
             exp = {"config": cfg, "env_id": "SyntheticVectorHumanoid", "optimizer": {"args": {"stepsize": LR}, "type": "adam"},
                    "policy": {"args": {"ac_bins": "continuous:", "ac_noise_std": 0.0, "connection_type": "ff",
@@ -285,7 +287,7 @@ def run_gpu_ref_proxy(args, emit, ClockSampler):
         batched matmul, the dense layers as batched mat-vec (gym_tensorflow/ops/indexedmatmul.cpp:169-202: SgemmBatched over
         host-built pointer arrays; models/base.py:54-99) -- i.e. every member streams its own 16.2 MB of weights per tick
         (no antithetic sharing, no split of theta and noise),
-      * argmax on the device, synthetic observations / rewards resident in HBM (as in the b200 arm's `value`).
+      * argmax on the device, synthetic observations / rewards resident in HBM (as in the gpu arm's `value`).
     What it leaves out (all in the reference's disfavour): TF op dispatch, the per-call host pointer-array build + H2D,
     the CPU env thread pool, the master's numpy update.  So it is a LOWER bound on the reference schedule's time here."""
     import torch

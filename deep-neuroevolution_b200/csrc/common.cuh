@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libdne.so (sm_100a only).
+// common.cuh -- shared helpers for libdne.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,8 +8,8 @@
 
 #include "../../include/dne.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libdne is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libdne is written for sm_90a (H100) only"
 #endif
 
 #define DNE_MAX_PREP 16
@@ -67,7 +67,7 @@ void dne_set_error(const char* fmt, ...);
 // ---- programmatic dependent launch (PDL) of the tick's kernel chain -----------------------------------------------
 // conv1 -> conv2 -> conv3 -> theta GEMM -> noise GEMV -> combine+head run back to back on one stream.  Kernels 2..6 are
 // launched with cudaLaunchAttributeProgrammaticStreamSerialization: every kernel of the chain calls pdl_trigger() first
-// thing (the NEXT launch may be scheduled as soon as all CTAs of this grid have started), sets itself up (barriers, TMEM,
+// thing (the NEXT launch may be scheduled as soon as all CTAs of this grid have started), sets itself up (barriers,
 // weight prefetch: nothing that an upstream kernel of the tick writes) and calls pdl_wait() before the first access to
 // upstream data or to any global buffer it writes.  pdl_wait() returns when the previous grid has completed and flushed --
 // which itself waited for ITS predecessor, so completion is transitive along the chain.  The launch latency and the

@@ -1,70 +1,62 @@
-// conv_s2d.cu -- the member convolutions as shifted-window implicit GEMMs on tcgen05 (TMEM accumulators), A operand
-// fed by TMA, persistent warp-specialised CTAs.  Replaces conv_tc_kernel (tc_conv.cu) on the per-tick path.
+// conv_s2d.cu -- the member convolutions as shifted-window implicit GEMMs on the Hopper tensor cores (wgmma, accumulators
+// in the registers of two MMA warpgroups), A operand fed by TMA, persistent warp-specialised CTAs.  Replaces
+// conv_tc_kernel (tc_conv.cu) on the per-tick path.
 //
 // Same contraction as the reference's per-member conv2d (policies.py:321-327,451-453; models/dqn.py:41-45,
 // models/base.py:54-75: extract_image_patches + batched matmul; TF 'SAME', NHWC, HWIO):
 //   out[m][n] = act( sum_{ky,kx,ci} in[oy*S-P+ky][ox*S-P+kx][ci] * w[ky][kx][ci][n] + b[n] ),   w = theta + s*noise[idx:]
 //
-// What changed against conv_tc_kernel (r01: 126 us per 256-slot tick, tensor pipe 13-18 %):
+// What differs from conv_tc_kernel:
 //   * NO im2col copy.  The (zero padded) input is space-to-depth'ed by the stride S, which turns the KSxKS/stride-S
 //     convolution into a (KS/S)x(KS/S)/stride-1 convolution over a W x W pixel grid with S*S*CIN channels.  The image
-//     is kept in shared memory as channel-octet planes  img[plane][pixel][8 x fp16]  -- which IS the UMMA K-major no-swizzle
-//     canonical layout of a matrix whose rows are the pixels (8 pixels = one 128-byte core matrix, SBO = 128, next
-//     channel octet LBO = PIXP*16 bytes; a 16-byte row holds 8 fp16 channels).  Output position m = oy*W + ox reads pixel m + ty*W + tx for tap (ty, tx): the
-//     SAME image at a start address shifted by (ty*W+tx)*16 bytes.  One smem descriptor per (tap, channel octet, M tile);
-//     rows with ox >= HOUT are junk accumulator rows that the epilogue skips (dev/tc_window.cu is the hardware
-//     self-test of this addressing; tests/test_gpu_tc.py::test_tcgen05_shifted_window_operand).
-//     Staging traffic per member drops from KS*KS/(S*S) x the input (conv3: 9x) to 1x, and for every layer but the first
-//   * the image is not staged by threads at all: the PRODUCING layer's epilogue writes the next layer's image (already
-//     space-to-depth'ed, zero padded, split into fp16 hi / lo planes) to global memory in exactly the shared-memory
-//     layout, and a producer thread brings it in with cp.async.bulk (TMA), one channel-octet group per mbarrier, so the
-//     MMAs of member i overlap the loads of member i+1 (a group's buffer is released by tcgen05.commit).
-//     The first layer converts the uint8 frame (exact in fp16: one plane, /255 applied to the accumulator).
-//   * the member's raw weights are not fetched by the staging threads either (r02 first version: one serialized global
-//     round trip per 16 KB chunk, 35-47K cycles per member against 6-16K of MMA work): a second producer thread streams
-//     the chunk's theta rows and noise rows (16-byte aligned supersets of the arbitrarily aligned slices) with
-//     cp.async.bulk into the ring stage that will hold the operand tile, NSTB chunks deep; converter warps read the raw
-//     rows from shared memory, perturb + split, and overwrite the SAME stage with the canonical [B_hi ; B_lo] tile.
-//   * persistent CTAs (one per SM), three pipelines: A groups (TMA or staging warps <-> MMA), B ring (staging warps
-//     <-> MMA: the member's perturbed weights fl(theta + fl(s*noise)) split h0/h1, [B_h0; B_h1] stacked along N), and a
-//     double-buffered TMEM accumulator (MMA <-> epilogue warps), so staging, MMA issue and epilogue of consecutive
-//     members overlap.
-//   * arithmetic: tcgen05.mma kind::f16 on 2 x fp16 splits (tc05.cuh: x = h0 + h1*2^-11, 22 significand bits; uint8 pixels
-//     are exact in fp16 and need one plane) -- twice the MAC rate and half the operand bytes of the 3xTF32 formulation the
-//     first r02 version used (the kernels are MMA bound): main accumulator D0 = A_h0*B_h0, correction accumulator
-//     D1 = A_h0*B_h1 + A_h1*B_h0 (B_h0 and B_h1 stacked along N: one N = 2*COUT MMA + one N = COUT MMA per K = 16 step),
-//     result = D0 + 2^-11 * D1.  fp16 x fp16 products are exact in the fp32 accumulators.
+//     is kept in shared memory as channel-octet planes  img[plane][pixel][8 x fp16]  -- which IS the wgmma K-major
+//     no-swizzle canonical layout of a matrix whose rows are the pixels (8 pixels = one 128-byte core matrix, SBO = 128,
+//     next channel octet LBO = PIXP*16 bytes; a 16-byte row holds 8 fp16 channels).  Output position m = oy*W + ox reads
+//     pixel m + ty*W + tx for tap (ty, tx): the SAME image at a start address shifted by (ty*W+tx)*16 bytes.  One smem
+//     descriptor per (tap, channel octet, m64 tile); rows with ox >= HOUT are junk accumulator rows that the epilogue
+//     skips (dev/tc_window.cu is the hardware self-test of this addressing; tests/test_gpu_tc.py::test_tcgen05_shifted_window_operand).
+//     Staging traffic per member drops from KS*KS/(S*S) x the input (conv3: 9x) to 1x.
+//   * for every layer but the first the image is not staged by threads at all: the PRODUCING layer's epilogue writes the
+//     next layer's image (already space-to-depth'ed, zero padded, split into fp16 hi / lo planes) to global memory in
+//     exactly the shared-memory layout, and a producer thread brings it in with cp.async.bulk (TMA), one channel-octet
+//     group per mbarrier, so the MMAs of member i overlap the loads of member i+1 (a group's buffer is released by the
+//     MMA warps once their wgmmas reading it have completed).  The first layer converts the uint8 frame (exact in fp16:
+//     one plane, /255 applied to the accumulator).
+//   * the member's raw weights are not fetched by the staging threads either: a second producer thread streams the
+//     chunk's theta rows and noise rows (16-byte aligned supersets of the arbitrarily aligned slices) with cp.async.bulk
+//     into the ring stage that will hold the operand tile, NSTB chunks deep; converter warps read the raw rows from shared
+//     memory, perturb + split, and overwrite the SAME stage with the canonical [B_hi ; B_lo] tile.
+//   * persistent CTAs (one per SM), warpgroup-specialised: two MMA warpgroups (each owns every other m64 tile of the
+//     member's rows and runs the fused epilogue from its registers), one converter warpgroup, and a producer warpgroup (image
+//     TMA warp + weight TMA warp).  setmaxnreg moves registers from the converter / producer warpgroups to the MMA
+//     warpgroups, whose accumulators take 128 registers per thread.  A groups (TMA or converters <-> MMA) and the B ring
+//     (converters <-> MMA) run ahead of the MMA warpgroups, so staging of member i+1 overlaps the MMAs and epilogue of i.
+//   * arithmetic: wgmma kind f16 on 2 x fp16 splits (wgmma.cuh: x = h0 + h1*2^-11, 22 significand bits; uint8 pixels
+//     are exact in fp16 and need one plane) -- twice the MAC rate and half the operand bytes of a 3xTF32 formulation:
+//     main accumulator D0 = A_h0*B_h0, correction accumulator D1 = A_h0*B_h1 + A_h1*B_h0 (B_h0 and B_h1 stacked along N:
+//     one N = 2*COUT MMA + one N = COUT MMA per K = 16 step), result = D0 + 2^-11 * D1.  fp16 x fp16 products are exact
+//     in the fp32 accumulators.
 #include "common.cuh"
 #include "forward.cuh"
 #include "epilogue.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
-using namespace tc05;
-
-#ifdef DNE_S2D_TRACE       // dev timeline of CTA 0 (make EXTRA=-DDNE_S2D_TRACE OUT=...; tools/s2d_trace.py); never in the product build
-__device__ long long g_s2d_trace[3][512];
-extern "C" int dne_debug_s2d_trace(long long* host_out) {
-    return cudaMemcpyFromSymbol(host_out, g_s2d_trace, sizeof(g_s2d_trace)) == cudaSuccess ? 0 : -3;
-}
-#define S2D_TR(cond, i) do { if (blockIdx.x == 0 && (cond) && (i) < 512) g_s2d_trace[TRL][(i)] = clock64(); } while (0)
-#define S2D_EV(it, g, e) (16 + (((it) * 16 + (g)) * 8 + (e)))
-#else
-#define S2D_TR(cond, i) do { } while (0)
-#define S2D_EV(it, g, e) 0
-#endif
+using namespace wg;
 
 namespace {
 
-constexpr int S2D_STAGE_WARPS = 8;                         // B (and uint8 A) staging
-constexpr int S2D_EPI_WARPS = 8;                           // two per TMEM lane quarter (they split the column groups)
-constexpr int S2D_STAGE_THREADS = S2D_STAGE_WARPS * 32;
-constexpr int S2D_EPI_THREADS = S2D_EPI_WARPS * 32;
-constexpr int S2D_THREADS = S2D_STAGE_THREADS + S2D_EPI_THREADS + 96;   // + MMA warp + image producer warp + weight producer warp
+// warpgroup roles: 0-1 MMA + epilogue, 2 converters (B tiles; first layer: also the uint8 frame), 3 producers (warp 12:
+// image / frame TMA, warp 13: weight TMA; warps 14-15 idle)
+constexpr int S2D_MMA_THREADS = 256;
+constexpr int S2D_CONV_WARPS = 4;
+constexpr int S2D_CONV_THREADS = S2D_CONV_WARPS * 32;
+constexpr int S2D_THREADS = 512;
+constexpr int S2D_REGS_MMA = 176, S2D_REGS_AUX = 80;        // setmaxnreg split: 2 * 176 + 2 * 80 = 512 = 65536 / 128
 constexpr int S2D_FRAME_BYTES = 84 * 84 * 4;                            // the uint8 frame stack of the first layer
 constexpr int S2D_FRAME_STRIDE = (S2D_FRAME_BYTES + 127) / 128 * 128;
 constexpr int S2D_MAX_GROUPS = 8;
 constexpr int S2D_MAX_BST = 8;       // ring depth: a stage cycles through TMA latency -> conversion -> MMA, ~4.6K cycles (conv3): 4 stages were the limit
-constexpr int S2D_SMEM_BUDGET = 226 * 1024;
+constexpr int S2D_SMEM_BUDGET = 222 * 1024;                 // + static shared memory <= 227 KB
 
 constexpr int cmin(int a, int b) { return a < b ? a : b; }
 constexpr int cmax(int a, int b) { return a > b ? a : b; }
@@ -98,9 +90,12 @@ struct S2dCfg {
     static constexpr int W = G.W, KT = G.KT, NTAP = KT * KT, NG = G.NG, PIXP = G.PIXP, LBO_A = G.LBO;
     static constexpr int PARTS = G.PARTS, GROUP_BYTES = G.GROUP_BYTES, IMG_BYTES = G.IMG_BYTES;
     static constexpr int MMAX = (HOUT - 1) * (W + 1);            // largest valid accumulator row
-    static constexpr int MT = MMAX / 128 + 1;                    // M tiles of 128 rows
+    static constexpr int MT = MMAX / 64 + 1;                     // m64 tiles; MMA warpgroup w owns tiles w, w + 2, ...
+    static constexpr int NTW = (MT + 1) / 2;                     // tiles of MMA warpgroup 0 (warpgroup 1: MT / 2)
+    static constexpr int ACC = COUT / 2;                         // accumulator floats per thread and tile, main and correction each
+    static_assert(2 * NTW * ACC <= 128, "accumulators exceed the MMA warpgroups' register budget");
     static constexpr int MAXOFF = (KT - 1) * (W + 1);
-    static constexpr int REACH = MT * 128 + MAXOFF;              // pixels a descriptor may touch from a plane start
+    static constexpr int REACH = MT * 64 + MAXOFF;               // pixels a descriptor may touch from a plane start
     static constexpr int SLACK = REACH > PIXP ? ((REACH - PIXP) * 16 + 127) / 128 * 128 : 0;
     static constexpr int A_REGION = IMG_BYTES + SLACK;
     static constexpr int LBO_B = 2 * COUT * 16;                  // [B_h0 ; B_h1] stacked along N, 8 fp16 k values per row
@@ -118,13 +113,10 @@ struct S2dCfg {
     static constexpr int NSTB = cmin(S2D_MAX_BST, (S2D_SMEM_BUDGET - A_REGION - FRAME_REGION - 256) / BST_BYTES);
     static_assert(NSTB >= 2, "shared memory: B ring too shallow");
     static constexpr int SMEM_BYTES = A_REGION + NSTB * BST_BYTES + FRAME_REGION + 256;
-    static constexpr int ACC_COLS = MT * 2 * COUT;               // one accumulator buffer: per M tile [main | correction]
-    static constexpr int TMEM_COLS = 2 * ACC_COLS <= 32 ? 32 : 2 * ACC_COLS <= 64 ? 64 : 2 * ACC_COLS <= 128 ? 128 : 2 * ACC_COLS <= 256 ? 256 : 512;
-    static_assert(2 * ACC_COLS <= 512, "TMEM: double-buffered accumulators do not fit");
     static constexpr int B_UNITS = COUT * TPC * 2;               // (column n, k octet) units per chunk
     // converter groups: chunk c is converted by group c % NGRP (independent streams hide the per-chunk hand-off latency)
     static constexpr int NGRP = 2;
-    static constexpr int WPG = S2D_STAGE_WARPS / NGRP, TG = 32 * WPG;
+    static constexpr int WPG = S2D_CONV_WARPS / NGRP, TG = 32 * WPG;
     static constexpr int B_UPT = (B_UNITS + TG - 1) / TG;
     static_assert(TG % COUT == 0 && NCH % NGRP == 0, "B unit map: a thread keeps its column; groups alternate chunks");
     static_assert(!IN_U8 || NCPG == 1, "the uint8 frame is staged per channel group by the group's (only) chunk");
@@ -141,6 +133,14 @@ struct S2dOut {
 };
 
 // ------------------------------------------------------------------------------------------------------------------
+// the pair (v0, v1) of fp32 values -> one 4-byte fp16 word of the hi plane and one of the (scaled) lo plane
+__device__ __forceinline__ void store_split_pair(uint4* p_hi, uint4* p_lo, int word, float v0, float v1) {
+    uint32_t hi, lo;
+    split_f16x2(v0, v1, hi, lo);
+    reinterpret_cast<uint32_t*>(p_hi)[word] = hi;
+    reinterpret_cast<uint32_t*>(p_lo)[word] = lo;
+}
+
 template <int CIN, int COUT, int KS, int S, int HIN, int HOUT, int PAD, bool IN_U8>
 __global__ void __launch_bounds__(S2D_THREADS, 1)
 conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict__ in_base, int64_t in_slot_stride,
@@ -150,97 +150,166 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
     // index, scale, active flag, BN statistics), v indexes the input / output buffers.  in_mod > 0: the first layer's frames
     // are shared by all members (frame v % in_mod).
     using Cfg = S2dCfg<CIN, COUT, KS, S, HIN, HOUT, PAD, IN_U8>;
-    constexpr int NG = Cfg::NG, NSTB = Cfg::NSTB, MT = Cfg::MT, NTAP = Cfg::NTAP, W = Cfg::W, KT = Cfg::KT;
+    constexpr int NG = Cfg::NG, NSTB = Cfg::NSTB, MT = Cfg::MT, NTW = Cfg::NTW, W = Cfg::W, KT = Cfg::KT;
     constexpr int TPC = Cfg::TPC, NCPG = Cfg::NCPG, NCH = Cfg::NCH;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
-    __shared__ uint64_t a_full[NG], a_empty[NG], raw_full[NSTB], b_full[NSTB], b_empty[NSTB], acc_full[2], acc_empty[2];
+    __shared__ uint64_t a_full[NG], a_empty[NG], raw_full[NSTB], b_full[NSTB], b_empty[NSTB];
     __shared__ uint64_t frame_full[2], frame_empty[2];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(16) float s_bias[COUT], s_mean[COUT], s_inv[COUT], s_gamma[COUT], s_beta[COUT];   // per-channel epilogue
+    // per-channel epilogue parameters, double buffered by member parity
+    __shared__ __align__(16) float s_bias[2][COUT], s_mean[2][COUT], s_inv[2][COUT], s_gamma[2][COUT], s_beta[2][COUT];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     pdl_trigger();                                               // common.cuh: the next kernel of the tick may be scheduled
-#ifdef DNE_S2D_TRACE
-    constexpr int TRL = IN_U8 ? 0 : (KS == 4 ? 1 : 2);
-#endif
-    S2D_TR(tid == 0, 0);
     const uint32_t sA = smem_u32(smem), sB = sA + Cfg::A_REGION;
     uint8_t* const gB = smem + Cfg::A_REGION;                                    // generic view of the ring (bulk copies)
     uint8_t* const gFrame = gB + NSTB * Cfg::BST_BYTES;
 
-    if (warp == 0) tmem_alloc(&tmem_base_s, Cfg::TMEM_COLS);
-    if (tid == 32) {
+    if (tid == 0) {
         for (int i = 0; i < NG; ++i) {
             mbar_init(&a_full[i], IN_U8 ? Cfg::WPG : 1);          // the converting group (uint8 frame) or the TMA producer
-            mbar_init(&a_empty[i], 1);                            // tcgen05.commit
+            mbar_init(&a_empty[i], S2D_MMA_THREADS);              // every MMA thread arrives (no divergent branch between wgmmas)
         }
         for (int i = 0; i < NSTB; ++i) {
             mbar_init(&raw_full[i], 1);                           // weight producer (expect_tx)
             mbar_init(&b_full[i], Cfg::WPG);                      // the warps of the converting group
-            mbar_init(&b_empty[i], 1);
+            mbar_init(&b_empty[i], S2D_MMA_THREADS);
         }
         for (int i = 0; i < 2; ++i) {
             mbar_init(&frame_full[i], 1);
-            mbar_init(&frame_empty[i], S2D_STAGE_WARPS);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&acc_empty[i], S2D_EPI_WARPS);
+            mbar_init(&frame_empty[i], S2D_CONV_WARPS);
         }
         fence_mbar_init();
     }
-    fence_before_thread_sync();
     __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = tmem_base_s;
-    S2D_TR(tid == 0, 1);
+    if (warp < 8) regs_inc<S2D_REGS_MMA>();                      // warpgroup-uniform: every warp of a warpgroup runs the same one
+    else regs_dec<S2D_REGS_AUX>();
 
-    if (warp == S2D_STAGE_WARPS + S2D_EPI_WARPS) {
-        // ================= MMA warp: converged loop, one elected lane issues (tc05.cuh: elect_one) =================
-        constexpr uint32_t IDESC2 = idesc_f16(128, 2 * COUT), IDESC1 = idesc_f16(128, COUT);
-        const uint64_t dA0 = smem_desc(sA, Cfg::LBO_A, 128), dB0 = smem_desc(sB, Cfg::LBO_B, 128);
+    if (warp < 8) {
+        // ============ MMA warpgroups: wgmma into registers, then the fused epilogue of the member ============
+        const int w = warp >> 2, wq = warp & 3;
+        const int et = tid;                                      // 0 .. 255
+        constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
+        const int act = epi.act;
+        const bool bn = epi.bn != DNE_BN_NONE;
+        // main and correction accumulators are separate register blocks: a wgmma into a sub-block of another wgmma's
+        // accumulators leaves ptxas without registers for the pipeline and serialises every wgmma
+        float acc[NTW][Cfg::ACC], cor[NTW][Cfg::ACC];
         uint32_t cb = 0, it = 0;
+        pdl_wait();                                              // before the first global write (the zero padding below)
         for (int slot = blockIdx.x; slot < n_slots; slot += gridDim.x) {
-            if (!slot_active(sa, slot / vdiv)) continue;
-            const uint32_t buf = it & 1;
-            mbar_wait(&acc_empty[buf], ((it >> 1) & 1) ^ 1);     // the epilogue has drained this accumulator buffer
-            fence_after_thread_sync();
-            const uint32_t d0 = tmem_base + buf * Cfg::ACC_COLS;
+            const int ms = slot / vdiv;
+            if (!slot_active(sa, ms)) continue;
+            const uint32_t pb = it & 1;
+            {
+                const float* th = slot_theta(sa, ms);
+                const int64_t idx = sa.noise_idx[ms];
+                const float s = sa.scale[ms];
+                for (int c = et; c < COUT; c += S2D_MMA_THREADS) {
+                    const ChanEpi ce = make_chan_epi(sa, epi, ms, COUT, c, th, idx, s);
+                    s_bias[pb][c] = ce.bias; s_mean[pb][c] = ce.mean; s_inv[pb][c] = ce.inv; s_gamma[pb][c] = ce.gamma; s_beta[pb][c] = ce.beta;
+                }
+            }
+            float* outp = so.base + slot * so.slot_stride;
+            if (so.next_img) {
+                // zero padding of the next layer's image: pixels (Y, X) of its padded grid that no output maps to
+                const int nHP = so.nHP, no = COUT / 8;
+                for (int b = et; b < nHP * nHP; b += S2D_MMA_THREADS) {
+                    const int Y = b / nHP, X = b - Y * nHP;
+                    if (Y >= so.nPADB && Y < so.nPADB + HOUT && X >= so.nPADB && X < so.nPADB + HOUT) continue;
+                    const int pix = (Y / so.nS) * so.nW + (X / so.nS), pp = (Y % so.nS) * so.nS + (X % so.nS);
+                    for (int q = 0; q < no; ++q) {
+                        const int co = pp * no + q;                                   // channel octet of the next image
+                        uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
+                        p[0] = make_uint4(0u, 0u, 0u, 0u);
+                        p[(size_t)2 * so.nPIXP] = make_uint4(0u, 0u, 0u, 0u);
+                    }
+                }
+            }
+            // ---- main loop: one chunk = TPC taps x 16 channels of one channel group ----
             for (int c = 0; c < NCH; ++c, ++cb) {
                 const int g = c / NCPG, tc = c - g * NCPG;
                 const uint32_t st = cb % NSTB;
                 if (tc == 0) mbar_wait(&a_full[g], it & 1);
-                S2D_TR(lane == 0 && it < 2 && c < 16, S2D_EV(it, c, 4));
                 mbar_wait(&b_full[st], (cb / NSTB) & 1);
-                S2D_TR(lane == 0 && it < 2 && c < 16, S2D_EV(it, c, 5));
-                fence_after_thread_sync();
-                if (elect_one()) {
-                    const uint64_t dAg = dA0 + (uint64_t)((g * Cfg::GROUP_BYTES) >> 4);
-                    const uint64_t dBs = dB0 + (uint64_t)((st * Cfg::BST_BYTES) >> 4);
+                wgmma_fence();
 #pragma unroll
-                    for (int tl = 0; tl < TPC; ++tl) {
-                        const int tap = tc * TPC + tl;
-                        const int toff = (tap / KT) * W + (tap % KT);
-                        const uint64_t dB = dBs + (uint64_t)((tl * 2 * Cfg::LBO_B) >> 4);
+                for (int tl = 0; tl < TPC; ++tl) {
+                    const int tap = tc * TPC + tl;
+                    const int toff = (tap / KT) * W + (tap % KT);
+                    const uint64_t dB = smem_desc(sB + st * Cfg::BST_BYTES + tl * 2 * Cfg::LBO_B, Cfg::LBO_B, 128);
 #pragma unroll
-                        for (int mt = 0; mt < MT; ++mt) {
-                            const uint64_t dAh = dAg + (uint64_t)(mt * 128 + toff);         // 16-byte units == pixels
-                            const uint32_t d = d0 + mt * 2 * COUT;
-                            mma_f16(d, dAh, dB, IDESC2, (c | tl) != 0);                                       // A_h0 * [B_h0 ; B_h1]
-                            if (!IN_U8) mma_f16(d + COUT, dAh + (uint64_t)((2 * Cfg::LBO_A) >> 4), dB, IDESC1, 1);   // A_h1 * B_h0 -> correction
+                    for (int j = 0; j < NTW; ++j) {
+                        // no branch around the wgmmas (a warp-divergent path serialises them): with an odd tile count,
+                        // warpgroup 1 recomputes the last tile into an accumulator its epilogue skips
+                        const int t = min(w + 2 * j, MT - 1);
+                        const uint64_t dA = smem_desc(sA + g * Cfg::GROUP_BYTES + (t * 64 + toff) * 16, Cfg::LBO_A, 128);
+                        const uint32_t first = (c | tl) != 0;
+                        wgmma_f16<COUT>(acc[j], dA, dB, first);                                                  // A_h0 * B_h0
+                        wgmma_f16<COUT>(cor[j], dA, dB + (uint64_t)((COUT * 16) >> 4), first);                   // A_h0 * B_h1 -> correction
+                        if (!IN_U8) wgmma_f16<COUT>(cor[j], dA + (uint64_t)((2 * Cfg::LBO_A) >> 4), dB, 1);     // A_h1 * B_h0 -> correction
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                                 // the previous chunk's wgmmas have read their operands
+                if (c > 0) {
+                    const int pg = (c - 1) / NCPG;
+                    mbar_arrive(&b_empty[(cb - 1) % NSTB]);
+                    if ((c - 1) - pg * NCPG == NCPG - 1) mbar_arrive(&a_empty[pg]);
+                }
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int j = 0; j < NTW; ++j) {
+                fence_regs<Cfg::ACC>(acc[j]);
+                fence_regs<Cfg::ACC>(cor[j]);
+            }
+            mbar_arrive(&b_empty[(cb - 1) % NSTB]);
+            mbar_arrive(&a_empty[NG - 1]);
+            named_bar_sync(2, S2D_MMA_THREADS);                  // per-channel parameters (and padding) of this member ready
+            // ---- epilogue: registers -> (/255) + bias (+BN) + activation -> global ----
+#pragma unroll
+            for (int j = 0; j < NTW; ++j) {
+                const int t = w + 2 * j;
+                if (t >= MT) continue;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = t * 64 + wq * 16 + (lane >> 2) + 8 * h;
+                    const int oy = m / W, ox = m - oy * W;
+                    if (oy >= HOUT || ox >= HOUT) continue;
+#pragma unroll
+                    for (int i = 0; i < COUT / 8; ++i) {
+                        const int n = 8 * i + 2 * (lane & 3);
+                        float v[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float r = fmaf(cor[j][4 * i + 2 * h + e], F16_LO_INV, acc[j][4 * i + 2 * h + e]);   // main + 2^-11 * correction
+                            if (IN_U8) r *= IN_SCALE;
+                            r += s_bias[pb][n + e];
+                            if (bn) r = (r - s_mean[pb][n + e]) * s_inv[pb][n + e] * s_gamma[pb][n + e] + s_beta[pb][n + e];   // policies.py:322
+                            v[e] = act == DNE_ACT_RELU ? fmaxf(r, 0.0f) : (act == DNE_ACT_TANH ? tanhf(r) : r);
+                        }
+                        if (!so.next_img) {
+                            *reinterpret_cast<float2*>(outp + (int64_t)(oy * HOUT + ox) * COUT + n) = make_float2(v[0], v[1]);
+                            if (so.xc) {
+                                const int ko = ((oy * HOUT + ox) * COUT + 8 * i) >> 3;
+                                uint4* xp = reinterpret_cast<uint4*>(so.xc) + ((int64_t)(slot >> 7) * so.xc_ko + ko) * 256 + (slot & 127);
+                                store_split_pair(xp, xp + 128, lane & 3, v[0], v[1]);
+                            }
+                        } else {
+                            const int Y = oy + so.nPADB, X = ox + so.nPADB;
+                            const int pix = (Y / so.nS) * so.nW + (X / so.nS);
+                            const int pp = (Y % so.nS) * so.nS + (X % so.nS);
+                            const int co = pp * (COUT / 8) + i;                             // channel octet of the next image
+                            uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
+                            store_split_pair(p, p + (size_t)2 * so.nPIXP, lane & 3, v[0], v[1]);
                         }
                     }
-                    mma_commit(&b_empty[st]);
-                    if (tc == NCPG - 1) mma_commit(&a_empty[g]);
-                    if (c == NCH - 1) mma_commit(&acc_full[buf]);
                 }
-                __syncwarp();
-                S2D_TR(lane == 0 && it < 2 && c < 16, S2D_EV(it, c, 6));
             }
             ++it;
         }
-    } else if (warp == S2D_STAGE_WARPS + S2D_EPI_WARPS + 1) {
+    } else if (warp == 12) {
         // ================= image producer (TMA): the member's image, one channel-octet group per bulk copy; =================
         // ================= first layer: the member's raw uint8 frame (double buffered)                      =================
         if (lane == 0) {
@@ -266,7 +335,7 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
                 ++it;
             }
         }
-    } else if (warp == S2D_STAGE_WARPS + S2D_EPI_WARPS + 2) {
+    } else if (warp == 13) {
         // ================= weight producer (TMA): raw theta rows + raw noise rows of every chunk, NSTB chunks deep =================
         if (lane == 0) {
             uint32_t cb = 0;
@@ -280,7 +349,6 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
                     const int g = c / NCPG, tc = c - g * NCPG;
                     const uint32_t st = cb % NSTB;
                     mbar_wait(&b_empty[st], ((cb / NSTB) & 1) ^ 1);
-                    S2D_TR(cb < 2 * NCH && c < 16, S2D_EV(cb / NCH, c, 0));
                     mbar_arrive_expect_tx(&raw_full[st], Cfg::RAW_BYTES);
                     uint8_t* dst = gB + st * Cfg::BST_BYTES;
                     const int cp = 16 * g, pp = cp / CIN, ci = cp % CIN, py = pp / S, px = pp % S;
@@ -292,23 +360,23 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
                         bulk_g2s(dst + tl * Cfg::PIECE_STRIDE, th + (int64_t)kk * COUT - a_t, Cfg::PIECE_STRIDE, &raw_full[st]);
                         bulk_g2s(dst + (TPC + tl) * Cfg::PIECE_STRIDE, nz + (int64_t)kk * COUT - a_n, Cfg::PIECE_STRIDE, &raw_full[st]);
                     }
-                    S2D_TR(cb < 2 * NCH && c < 16, S2D_EV(cb / NCH, c, 1));
                 }
             }
         }
-    } else if (warp < S2D_STAGE_WARPS) {
+    } else if (warp < 12) {
         // ================= converter warps: raw rows -> perturbed, split [B_hi ; B_lo] tile, in place =================
         // =================                  (first layer: also the uint8 frame -> image planes)       =================
         constexpr int TG = Cfg::TG, NGRP = Cfg::NGRP;
-        const int grp = warp / Cfg::WPG, tg = tid - grp * TG;
+        const int ct = tid - S2D_MMA_THREADS;                    // 0 .. S2D_CONV_THREADS - 1
+        const int grp = ct / TG, tg = ct - grp * TG;
         // zero fill, once: the uint8 variant relies on the zero padding of its image never being overwritten (the
         // converter warps are its only writers); the TMA-fed variants only need finite values in the slack behind the last
         // plane, which is read into junk accumulator rows.  Only the converter warps wait for it.
         {
             constexpr int Z0 = IN_U8 ? 0 : Cfg::IMG_BYTES, Z1 = Cfg::A_REGION;
-            for (int i = Z0 / 16 + tid; i < Z1 / 16; i += S2D_STAGE_THREADS) sts128(sA + i * 16, make_float4(0.f, 0.f, 0.f, 0.f));
+            for (int i = Z0 / 16 + ct; i < Z1 / 16; i += S2D_CONV_THREADS) sts128(sA + i * 16, make_float4(0.f, 0.f, 0.f, 0.f));
             fence_proxy_async_smem();
-            named_bar_sync(5, S2D_STAGE_THREADS);
+            named_bar_sync(1, S2D_CONV_THREADS);
         }
         const int n = tg % COUT;                                 // this thread's output channel in every unit
         constexpr int KQ_STEP = TG / COUT;
@@ -355,9 +423,7 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
                         if (c + NGRP >= NCH) mbar_arrive(&frame_empty[it & 1]);    // this warp's last read of the raw frame
                     }
                 }
-                S2D_TR(tg == 0 && it < 2 && c < 16, S2D_EV(it, c, 7));
                 mbar_wait(&raw_full[st], (cb / NSTB) & 1);
-                S2D_TR(tg == 0 && it < 2 && c < 16, S2D_EV(it, c, 2));
                 const uint32_t sBs = sB + st * Cfg::BST_BYTES;
                 float w[Cfg::B_UPT][8];
 #pragma unroll
@@ -384,123 +450,10 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&b_full[st]);
-                S2D_TR(tg == 0 && it < 2 && c < 16, S2D_EV(it, c, 3));
             }
-            ++it;
-        }
-    } else {
-        // ================= epilogue warps: TMEM -> (/255) + bias (+BN) + activation -> global =================
-        // warp ew: TMEM lane quarter ew & 3 (== warp % 4, the hardware rule), column-group parity ew >> 2
-        const int ew = warp - S2D_STAGE_WARPS, lq = ew & 3, half = ew >> 2;
-        const int et = tid - S2D_STAGE_THREADS;
-        constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
-        constexpr int NJ = COUT / 16;
-        const int act = epi.act;
-        const bool bn = epi.bn != DNE_BN_NONE;
-        uint32_t it = 0;
-        pdl_wait();                                              // before the first global write (the zero padding below)
-        for (int slot = blockIdx.x; slot < n_slots; slot += gridDim.x) {
-            const int ms = slot / vdiv;
-            if (!slot_active(sa, ms)) continue;
-            const float* th = slot_theta(sa, ms);
-            const int64_t idx = sa.noise_idx[ms];
-            const float s = sa.scale[ms];
-            for (int c = et; c < COUT; c += S2D_EPI_THREADS) {
-                const ChanEpi ce = make_chan_epi(sa, epi, ms, COUT, c, th, idx, s);
-                s_bias[c] = ce.bias; s_mean[c] = ce.mean; s_inv[c] = ce.inv; s_gamma[c] = ce.gamma; s_beta[c] = ce.beta;
-            }
-            float* outp = so.base + slot * so.slot_stride;
-            if (so.next_img) {
-                // zero padding of the next layer's image: pixels (Y, X) of its padded grid that no output maps to
-                const int nHP = so.nHP, no = COUT / 8;
-                for (int b = et; b < nHP * nHP; b += S2D_EPI_THREADS) {
-                    const int Y = b / nHP, X = b - Y * nHP;
-                    if (Y >= so.nPADB && Y < so.nPADB + HOUT && X >= so.nPADB && X < so.nPADB + HOUT) continue;
-                    const int pix = (Y / so.nS) * so.nW + (X / so.nS), pp = (Y % so.nS) * so.nS + (X % so.nS);
-                    for (int q = 0; q < no; ++q) {
-                        const int co = pp * no + q;                                   // channel octet of the next image
-                        uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
-                        p[0] = make_uint4(0u, 0u, 0u, 0u);
-                        p[(size_t)2 * so.nPIXP] = make_uint4(0u, 0u, 0u, 0u);
-                    }
-                }
-            }
-            named_bar_sync(2, S2D_EPI_THREADS);                  // per-channel parameters ready
-            const uint32_t buf = it & 1;
-            mbar_wait(&acc_full[buf], (it >> 1) & 1);
-            S2D_TR(et == 0 && it < 2, 2 + it);
-            fence_after_thread_sync();
-            const uint32_t t0 = tmem_base + buf * Cfg::ACC_COLS + ((uint32_t)(lq * 32) << 16);
-#pragma unroll 1
-            for (int q = half; q < MT * NJ; q += 2) {             // (M tile, 16-column group) work items of this warp
-                const int mt = q / NJ, n0 = (q - mt * NJ) * 16;
-                const int m = mt * 128 + lq * 32 + lane;
-                const int oy = m / W, ox = m - oy * W;
-                const bool valid = (oy < HOUT) && (ox < HOUT);
-                float v[16], v2[16];
-                __syncwarp();                                    // tcgen05.ld is .sync.aligned: the warp must be converged
-                tmem_ld16_async(t0 + (uint32_t)(mt * 2 * COUT + n0), v);
-                tmem_ld16_async(t0 + (uint32_t)(mt * 2 * COUT + COUT + n0), v2);
-                tmem_ld_wait();
-                if (valid) {
-#pragma unroll
-                    for (int x = 0; x < 16; x += 4) {
-                        const float4 b4 = *reinterpret_cast<const float4*>(&s_bias[n0 + x]);
-                        const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-                        for (int y = 0; y < 4; ++y) {
-                            float r = fmaf(v2[x + y], F16_LO_INV, v[x + y]);        // main + 2^-11 * correction accumulator
-                            if (IN_U8) r *= IN_SCALE;
-                            r += bb[y];
-                            if (bn) r = (r - s_mean[n0 + x + y]) * s_inv[n0 + x + y] * s_gamma[n0 + x + y] + s_beta[n0 + x + y];   // policies.py:322
-                            v[x + y] = act == DNE_ACT_RELU ? fmaxf(r, 0.0f) : (act == DNE_ACT_TANH ? tanhf(r) : r);
-                        }
-                    }
-                    if (!so.next_img) {
-                        float4* dst = reinterpret_cast<float4*>(outp + (int64_t)(oy * HOUT + ox) * COUT + n0);
-#pragma unroll
-                        for (int x = 0; x < 16; x += 4) dst[x / 4] = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
-                        if (so.xc) {
-                            const int ko0 = ((oy * HOUT + ox) * COUT + n0) >> 3;
-                            uint4* xp = reinterpret_cast<uint4*>(so.xc) + ((int64_t)(slot >> 7) * so.xc_ko + ko0) * 256 + (slot & 127);
-#pragma unroll
-                            for (int x = 0; x < 16; x += 8) {
-                                const float e[8] = {v[x], v[x + 1], v[x + 2], v[x + 3], v[x + 4], v[x + 5], v[x + 6], v[x + 7]};
-                                uint4 hi, lo;
-                                split_f16x8(e, hi, lo);
-                                xp[(x / 8) * 256] = hi;
-                                xp[(x / 8) * 256 + 128] = lo;
-                            }
-                        }
-                    } else {
-                        const int Y = oy + so.nPADB, X = ox + so.nPADB;
-                        const int pix = (Y / so.nS) * so.nW + (X / so.nS);
-                        const int pp = (Y % so.nS) * so.nS + (X % so.nS);
-#pragma unroll
-                        for (int x = 0; x < 16; x += 8) {
-                            const int co = pp * (COUT / 8) + (n0 + x) / 8;            // channel octet of the next image
-                            const float e[8] = {v[x], v[x + 1], v[x + 2], v[x + 3], v[x + 4], v[x + 5], v[x + 6], v[x + 7]};
-                            uint4 hi, lo;
-                            split_f16x8(e, hi, lo);
-                            uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
-                            p[0] = hi;
-                            p[(size_t)2 * so.nPIXP] = lo;
-                        }
-                    }
-                }
-            }
-            fence_before_thread_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-            S2D_TR(et == 0 && it < 2, 4 + it);
-            named_bar_sync(2, S2D_EPI_THREADS);                  // per-channel parameters reusable
             ++it;
         }
     }
-    fence_before_thread_sync();
-    __syncthreads();
-    S2D_TR(tid == 0, 6);
-    if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 template <int CIN, int COUT, int KS, int S, int HIN, int HOUT, int PAD, bool IN_U8>

@@ -1,4 +1,4 @@
-// dev.cuh -- helpers of the DEV library libdne_dev.so (self-tests and micro-probes of the tcgen05 / TMA plumbing).
+// dev.cuh -- helpers of the DEV library libdne_dev.so (self-tests of the wgmma / TMA plumbing).
 // Nothing here is part of the product ABI (include/dne.h); the product library libdne.so does not link it.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,37 +1,30 @@
-// tc_selftest.cu -- self-test of the tcgen05 plumbing (descriptors, TMEM alloc/ld, mbarrier commit, 3xTF32 split) used by
-// tests/test_gpu_tc.py.  Part of the DEV library libdne_dev.so, not of the product ABI (include/dne.h).
+// tc_selftest.cu -- self-test of the wgmma plumbing (descriptors, register accumulators, wgmma fence / commit / wait,
+// 3xTF32 split) used by tests/test_gpu_tc.py.  Part of the DEV library libdne_dev.so, not of the product ABI (include/dne.h).
 #include "dev.cuh"
-#include "../tc05.cuh"
-using namespace tc05;
-constexpr int TG_THREADS = 256;
+#include "../wgmma.cuh"
+using namespace wg;
 
 // =====================================================================================================
-// Self-test of the tcgen05 plumbing: C[128,N] = A[128,K] * B[N,K]^T with the same staging / descriptor / 3xTF32 code
-// path (single CTA).  Exposed by libdne_dev.so for tests/test_gpu_tc.py.
+// Self-test of the wgmma plumbing: C[128,N] = A[128,K] * B[N,K]^T with the same staging / descriptor / 3xTF32 code
+// path (single CTA = one warpgroup, two m64 tiles).  Exposed by libdne_dev.so for tests/test_gpu_tc.py.
 // =====================================================================================================
 template <int N>
 __global__ void __launch_bounds__(128) tc_gemm_test_kernel(const float* __restrict__ A, const float* __restrict__ B,
                                                            float* __restrict__ C, int K) {
     constexpr int KC = 32;
     constexpr int A_PLANE = 128 * 16, B_PLANE = N * 16;
-    constexpr int TCOLS = N < 32 ? 32 : N;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
     uint8_t* sA_hi = smem;
     uint8_t* sA_lo = sA_hi + (KC / 4) * A_PLANE;
     uint8_t* sB_hi = sA_lo + (KC / 4) * A_PLANE;
     uint8_t* sB_lo = sB_hi + (KC / 4) * B_PLANE;
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (warp == 0) tmem_alloc(&tmem_base_s, TCOLS);
-    if (tid == 32) { mbar_init(&bar, 1); fence_mbar_init(); }
-    fence_before_thread_sync();
-    __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = tmem_base_s;
-    constexpr uint32_t IDESC = idesc_tf32(128, N);
-    int phase = 0;
+    float acc[2][N / 2];
+#pragma unroll
+    for (int t = 0; t < 2; ++t)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[t][i] = 0.0f;
     for (int k0 = 0; k0 < K; k0 += KC) {
         for (int u = tid; u < 128 * (KC / 4); u += 128) {
             const int r = u % 128, q = u / 128;
@@ -51,34 +44,35 @@ __global__ void __launch_bounds__(128) tc_gemm_test_kernel(const float* __restri
         }
         fence_proxy_async_smem();
         __syncthreads();
-        if (tid == 0) {
-            fence_after_thread_sync();
-            for (int k8 = 0; k8 < KC / 8; ++k8) {
-                const uint64_t dAh = smem_desc(smem_u32(sA_hi) + 2 * k8 * A_PLANE, A_PLANE, 128);
-                const uint64_t dAl = smem_desc(smem_u32(sA_lo) + 2 * k8 * A_PLANE, A_PLANE, 128);
-                const uint64_t dBh = smem_desc(smem_u32(sB_hi) + 2 * k8 * B_PLANE, B_PLANE, 128);
-                const uint64_t dBl = smem_desc(smem_u32(sB_lo) + 2 * k8 * B_PLANE, B_PLANE, 128);
-                mma_tf32(tmem_base, dAh, dBh, IDESC, (k0 | k8) != 0);
-                mma_tf32(tmem_base, dAl, dBh, IDESC, 1);
-                mma_tf32(tmem_base, dAh, dBl, IDESC, 1);
+        wgmma_fence();
+#pragma unroll
+        for (int k8 = 0; k8 < KC / 8; ++k8) {
+            const uint64_t dBh = smem_desc(smem_u32(sB_hi) + 2 * k8 * B_PLANE, B_PLANE, 128);
+            const uint64_t dBl = smem_desc(smem_u32(sB_lo) + 2 * k8 * B_PLANE, B_PLANE, 128);
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {
+                const uint64_t dAh = smem_desc(smem_u32(sA_hi) + 2 * k8 * A_PLANE + t * 1024, A_PLANE, 128);
+                const uint64_t dAl = smem_desc(smem_u32(sA_lo) + 2 * k8 * A_PLANE + t * 1024, A_PLANE, 128);
+                wgmma_tf32<N>(acc[t], dAh, dBh, 1);
+                wgmma_tf32<N>(acc[t], dAl, dBh, 1);
+                wgmma_tf32<N>(acc[t], dAh, dBl, 1);
             }
-            mma_commit(&bar);
         }
-        mbar_wait(&bar, phase);            // synchronous version: wait before re-staging
-        phase ^= 1;
+        wgmma_commit();
+        wgmma_wait<0>();                   // synchronous version: wait before re-staging
+        fence_regs<N / 2>(acc[0]);
+        fence_regs<N / 2>(acc[1]);
+        __syncthreads();
     }
-    fence_after_thread_sync();
 #pragma unroll
-    for (int j = 0; j < N / 16; ++j) {
-        float v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + j * 16, v);
-        const int m = warp * 32 + lane;
+    for (int t = 0; t < 2; ++t)
 #pragma unroll
-        for (int x = 0; x < 16; ++x) C[(int64_t)m * N + j * 16 + x] = v[x];
-    }
-    fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, TCOLS);
+        for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = t * 64 + warp * 16 + (lane >> 2) + 8 * h, n = 8 * j + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(C + (int64_t)m * N + n) = make_float2(acc[t][4 * j + 2 * h], acc[t][4 * j + 2 * h + 1]);
+            }
 }
 
 extern "C" int dne_test_tc_gemm(const float* d_A, const float* d_B, float* d_C, int K, int N, void* stream) {
@@ -98,4 +92,3 @@ extern "C" int dne_test_tc_gemm(const float* d_A, const float* d_B, float* d_C, 
     DNE_LAUNCH_CHECK1();
     return DNE_OK;
 }
-

@@ -34,8 +34,8 @@ extern "C" int dne_ctx_create(int device, dne_ctx** out) {
     DNE_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     DNE_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
-        dne_set_error("dne_ctx_create: device %d is sm_%d%d; libdne is built for sm_100a (B200) only", device,
+    if (prop.major != 9 || prop.minor != 0) {
+        dne_set_error("dne_ctx_create: device %d is sm_%d%d; libdne is built for sm_90a (H100) only", device,
                       prop.major, prop.minor);
         return DNE_ERR_CUDA;
     }
@@ -73,7 +73,7 @@ extern "C" int dne_ctx_destroy(dne_ctx* ctx) {
     return DNE_OK;
 }
 
-// Runtime switches: "conv_tc" (1 = tcgen05 convolutions [default], 0 = fp32 SIMT convolutions).
+// Runtime switches: "conv_tc" (2 = shifted-window wgmma convolutions [default], 1 = im2col-staged wgmma, 0 = fp32 SIMT).
 extern "C" int dne_set_option(const char* name, int value) {
     DNE_CHECK_ARG(name, "name is null");
     if (strcmp(name, "conv_tc") == 0 && value >= 0 && value <= 2) { g_dne_conv_tc = value; return DNE_OK; }
@@ -152,7 +152,7 @@ extern "C" int dne_noise_bind(dne_ctx* ctx, const float* d_noise, int64_t count)
 // ---------------------------------------------------------------------------------------------------
 // forward planning: workspace carve-up
 // ---------------------------------------------------------------------------------------------------
-constexpr int PLAN_SM_COUNT = 148;   // B200; planning must not depend on a live device (ws query works on CPU)
+constexpr int PLAN_SM_COUNT = 132;   // H100 SXM; planning must not depend on a live device (ws query works on CPU)
 
 struct ForwardPlan {
     size_t x0_off;                         // normalised vector observations

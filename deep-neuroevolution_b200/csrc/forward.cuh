@@ -71,7 +71,7 @@ struct DenseHead {
     int32_t* actions;          // nullable
 };
 bool dne_head_fusable(const dne_layer_desc& L, const DensePlan& p, const dne_layer_desc& head, const DensePlan& hp);
-// TMA-fed shared-theta GEMM (theta_gemm_tma.cu): both operands pre-arranged in the UMMA canonical layout, split hi / lo
+// TMA-fed shared-theta GEMM (theta_gemm_tma.cu): both operands pre-arranged in the wgmma canonical layout, split hi / lo
 struct TgmOperands {
     const float* Xc;           // [m tile][k quad][hi|lo][128][4], written by the producing conv epilogue
     const float* Wc;           // [n tile][k quad][hi|lo][128][4], written by dne_theta_prepare
@@ -93,7 +93,7 @@ void dne_launch_ob_norm(const float* obs, const float* mean, const float* stdv, 
 int dne_launch_theta_gemm_tc(const float* X, int M, int K, int N, const float* W, int k_per_split, int n_split,
                              float* part, cudaStream_t st);
 
-// conv_s2d.cu: shifted-window implicit-GEMM convolutions (tcgen05, A operand by TMA), dne_set_option("conv_tc", 2) [default]
+// conv_s2d.cu: shifted-window implicit-GEMM convolutions (wgmma, A operand by TMA), dne_set_option("conv_tc", 2) [default]
 bool dne_s2d_supported(const dne_layer_desc& L, bool in_u8);
 size_t dne_s2d_image_bytes(const dne_layer_desc& L);
 int dne_launch_conv_layer_s2d(const SlotArgs& sa, const dne_layer_desc& L, const LayerEpi& epi, bool in_u8, const void* in,

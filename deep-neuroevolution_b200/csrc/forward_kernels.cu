@@ -22,7 +22,7 @@
 // Convolution as implicit GEMM, one member per blockIdx.y, BM output positions per CTA.
 //   A[m][k] = in[oy*S-PAD+ky][ox*S-PAD+kx][ci]   (TF SAME, NHWC; k = (ky,kx,ci), HWIO flat order: tf_util.py:135)
 //   B[k][n] = theta_w[k*COUT+n] + s*noise[idx+off_w+k*COUT+n]     built in shared memory per k-tile
-// fp32 SIMT register tile TM x TN.  (The tcgen05/TMEM version of this contraction replaces this kernel.)
+// fp32 SIMT register tile TM x TN.  (The wgmma version of this contraction replaces this kernel.)
 // ---------------------------------------------------------------------------------------------------
 constexpr int CONV_BK = 16;
 
@@ -626,7 +626,7 @@ static bool conv_is(const dne_layer_desc& L, int cin, int cout, int ks, int stri
 }
 
 // in_u8: the layer reads uint8 observations.  Returns 0 or DNE_ERR_UNSUP.
-int g_dne_conv_tc = 2;     // 2: shifted-window tcgen05 + TMA (conv_s2d.cu), 1: im2col-staged tcgen05 (tc_conv.cu), 0: fp32 SIMT
+int g_dne_conv_tc = 2;     // 2: shifted-window wgmma + TMA (conv_s2d.cu), 1: im2col-staged wgmma (tc_conv.cu), 0: fp32 SIMT
 
 int dne_launch_conv_layer(const SlotArgs& sa, const dne_layer_desc& L, const LayerEpi& epi, bool in_u8,
                           const void* in, int64_t in_slot_stride, int64_t in_img_stride, float* out,
@@ -735,8 +735,8 @@ int dne_launch_dense_layer(const dne_ctx* ctx, const SlotArgs& sa, const dne_lay
         return sm1 > sm2 ? sm1 : sm2;
     };
     if (p.Gt == 0) {
-        // TMA-fed tcgen05 GEMM when both operands are pre-arranged (dne_theta_prepare + conv_s2d epilogue); else
-        // thread-staged tensor cores (tcgen05, 3xTF32) when enabled, fp32 SIMT otherwise
+        // TMA-fed wgmma GEMM when both operands are pre-arranged (dne_theta_prepare + conv_s2d epilogue); else
+        // thread-staged tensor cores (wgmma, 3xTF32) when enabled, fp32 SIMT otherwise
         if (tgm && dne_launch_theta_gemm_tma(tgm->Xc, tgm->Wc, n_slots, K, N, p.k_per_split, p.n_split, part_theta, st) == 0) {
         } else if (!(g_dne_conv_tc && dne_launch_theta_gemm_tc(X, n_slots, K, N, sa.theta + L.off_w, p.k_per_split, p.n_split,
                                                         part_theta, st) == 0)) {

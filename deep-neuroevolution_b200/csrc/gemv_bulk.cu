@@ -15,9 +15,9 @@
 #include "common.cuh"
 #include "forward.cuh"
 #include "epilogue.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
-using namespace tc05;
+using namespace wg;
 
 int g_dne_gemv_bulk = 1;
 int g_dne_gemv_ctas_per_sm = 2;
@@ -183,11 +183,11 @@ gemv_bulk_kernel(SlotArgs sa, GemvSrc src, const float* __restrict__ X, int64_t 
                 for (int j = 0; j <= GB_RPR; ++j) xm[g][j] = xs[g][r0 + rl0 + j];        // xs index = 1 + (row - 1)
             mbar_wait(&full_bar[s], (it / n_stages) & 1);
             // explicit ld.shared (a C++ pointer into the re-aligned dynamic smem compiles to generic LD.E)
-            const uint32_t rows_a = tc05::smem_u32(stage_base) + s * GB_STAGE_BYTES + (rl0 * NQ + t) * 16;
+            const uint32_t rows_a = wg::smem_u32(stage_base) + s * GB_STAGE_BYTES + (rl0 * NQ + t) * 16;
             if (nr == RB) {
                 float4 v[GB_RPR];
 #pragma unroll
-                for (int j = 0; j < GB_RPR; ++j) v[j] = tc05::lds128(rows_a + j * NQ * 16);
+                for (int j = 0; j < GB_RPR; ++j) v[j] = wg::lds128(rows_a + j * NQ * 16);
 #pragma unroll
                 for (int j = 0; j < GB_RPR; ++j)
 #pragma unroll
@@ -212,7 +212,7 @@ gemv_bulk_kernel(SlotArgs sa, GemvSrc src, const float* __restrict__ X, int64_t 
             } else {
                 for (int j = 0; j < GB_RPR; ++j) {
                     if (rl0 + j < nr) {
-                        const float4 v = tc05::lds128(rows_a + j * NQ * 16);
+                        const float4 v = wg::lds128(rows_a + j * NQ * 16);
 #pragma unroll
                         for (int g = 0; g < G; ++g) {
                             acc[g][0] = fmaf(xm[g][j + 1], v.x, acc[g][0]);

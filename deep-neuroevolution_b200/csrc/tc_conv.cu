@@ -1,4 +1,4 @@
-// tc_conv.cu -- the member convolutions on the 5th-gen tensor cores (tcgen05.mma kind::tf32, accumulators in TMEM).
+// tc_conv.cu -- the member convolutions on the Hopper tensor cores (wgmma kind tf32, accumulators in registers).
 //
 // Same contraction as conv_kernel in forward_kernels.cu (implicit GEMM, one member per CTA):
 //   A[m][k] = im2col(input)            m = output position, k = (ky,kx,ci)      (TF SAME, NHWC)
@@ -9,33 +9,24 @@
 // D = Ahi*Bhi + Alo*Bhi + Ahi*Blo.  B_hi and B_lo are stacked along N in one tile, so Ahi*[Bhi;Blo] is ONE MMA (N = 2*COUT)
 // and Alo*Bhi a second one; uint8 inputs are staged as exact integers (no lo plane, /255 in the epilogue).
 // Operands are PRODUCED into shared memory by the perturb / im2col stage (they do not exist in global memory, so
-// there is nothing for TMA to fetch); the layout is the UMMA K-major no-swizzle canonical layout (tc05.cuh).
+// there is nothing for TMA to fetch); the layout is the wgmma K-major no-swizzle canonical layout (wgmma.cuh).
 // Warp-specialised mbarrier pipeline, no block barriers in the loop: TC_GROUPS staging groups of 128 threads (group g
-// owns shared-memory stage g and the k-chunks c = g mod TC_GROUPS) + one MMA warp that runs converged and issues from one
-// elected lane (tc05.cuh: elect_one); stage hand-off full[g] (staging warps arrive) / empty[g] (tcgen05.commit).
-// The staging warps then drain TMEM with tcgen05.ld for the fused epilogue.
+// owns shared-memory stage g and the k-chunks c = g mod TC_GROUPS) + two MMA warpgroups, each owning half of the M tile's
+// rows in its registers; stage hand-off full[g] (staging warps arrive) / empty[g] (MMA warps arrive once their wgmmas
+// of the stage have completed).  The MMA warpgroups then run the fused epilogue from their accumulator registers.
 #include "common.cuh"
 #include "forward.cuh"
 #include "epilogue.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
-using namespace tc05;
+using namespace wg;
 
-#ifdef DNE_CONV_TRACE
-__device__ long long g_conv_trace[1024];
-#define TRACE(cond, i) do { if (TRACE_ON && (cond)) g_conv_trace[i] = clock64(); } while (0)
-extern "C" int dne_debug_conv_trace(long long* host_out) {
-    return cudaMemcpyFromSymbol(host_out, g_conv_trace, sizeof(g_conv_trace)) == cudaSuccess ? 0 : -3;
-}
-#else
-#define TRACE(cond, i) do { } while (0)
-#endif
 #ifndef DNE_TC_GROUPS
-#define DNE_TC_GROUPS 3      // r01 A/B (tools/sweep_overlap.py): 3 groups (416 threads, 72 regs, no spills, 72 KB) >= 4 groups (56 regs, spills)
+#define DNE_TC_GROUPS 3      // staging groups of 128 threads (one shared-memory stage each)
 #endif
 constexpr int TC_GROUPS = DNE_TC_GROUPS;        // staging groups of 128 threads; group g owns smem stage g and stages chunks c = g (mod TC_GROUPS)
 constexpr int TC_THREADS = TC_GROUPS * 128;     // conv kernels: the staging warps ...
-constexpr int TC_BLOCK = TC_THREADS + 32;       // ... + one MMA-issuing warp (warp-specialised, mbarrier pipeline, no block barriers)
+constexpr int TC_BLOCK = TC_THREADS + 256;      // ... + two MMA warpgroups (warp-specialised, mbarrier pipeline, no block barriers)
 constexpr int TG_THREADS = 256;                 // theta GEMM / self-test
 
 template <int CIN, int COUT, int KS, int STRIDE, int HIN, int HOUT, int PAD, bool IN_U8, int MTC, int KC>
@@ -58,8 +49,7 @@ struct TcConvCfg {
     static constexpr int STAGE_BYTES = A_PLANES * A_BYTES + B_BYTES;
     static constexpr int NST = TC_GROUPS;                        // one shared-memory stage per staging group
     static constexpr int SMEM_BYTES = NST * STAGE_BYTES + 128;   // + alignment slack
-    static constexpr int ACC_COLS = MTC * 2 * COUT;
-    static constexpr int TMEM_COLS = (ACC_COLS <= 32) ? 32 : (ACC_COLS <= 64) ? 64 : (ACC_COLS <= 128) ? 128 : (ACC_COLS <= 256) ? 256 : 512;
+    static constexpr int ACC = COUT / 2;                          // accumulator floats per thread and m64 tile, per accumulator
     static constexpr int PASSES = ROWS / 32;                     // A rows per staging thread and chunk
     static constexpr int B_UNITS = COUT * (KC / 4);
     static constexpr int B_PER_THREAD = (B_UNITS + 127) / 128;
@@ -75,7 +65,7 @@ __device__ __forceinline__ void split_tf32_rn(float x, float& hi, float& lo) {
 }
 
 template <int CIN, int COUT, int KS, int STRIDE, int HIN, int HOUT, int PAD, bool IN_U8, int MTC, int KC>
-__global__ void __launch_bounds__(TC_BLOCK, 2)
+__global__ void __launch_bounds__(TC_BLOCK, 1)
 conv_tc_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict__ in_base, int64_t in_slot_stride,
                int64_t in_img_stride, float* __restrict__ out_base, int64_t out_slot_stride, int64_t out_img_stride) {
     using Cfg = TcConvCfg<CIN, COUT, KS, STRIDE, HIN, HOUT, PAD, IN_U8, MTC, KC>;
@@ -86,67 +76,83 @@ conv_tc_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict_
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     constexpr int NST = Cfg::NST;
     constexpr int STAGE_WARPS = TC_THREADS / 32;
-#ifdef DNE_CONV_TRACE        // dev timeline of one conv2 CTA (make EXTRA=-DDNE_CONV_TRACE; tools/conv_trace.py)
-    const bool TRACE_ON = CIN == 32 && COUT == 64 && blockIdx.x == 0 && blockIdx.y == 7;
-    TRACE(tid == 0, 0);
-    if (TRACE_ON && tid == 0) { unsigned long long ns; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(ns)); g_conv_trace[4] = (long long)ns; }
-#endif
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
-    __shared__ uint64_t full_bar[NST], empty_bar[NST], done_bar;
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full_bar[NST], empty_bar[NST];
     __shared__ ChanEpi epi_s[COUT];                              // per-channel epilogue parameters, built once per CTA
 
     const float* th = slot_theta(sa, slot);
     const int64_t idx = sa.noise_idx[slot];
     const float s = sa.scale[slot];
 
-    if (warp == 0) tmem_alloc(&tmem_base_s, Cfg::TMEM_COLS);
-    if (tid == 32) {
+    if (tid == 0) {
         for (int i = 0; i < NST; ++i) {
             mbar_init(&full_bar[i], 4);                          // one arrival per warp of the owning staging group
-            mbar_init(&empty_bar[i], 1);                         // tcgen05.commit of the MMA warp
+            mbar_init(&empty_bar[i], 8);                         // one arrival per MMA warp
         }
-        mbar_init(&done_bar, 1);
         fence_mbar_init();
     }
     if (tid < COUT) epi_s[tid] = make_chan_epi(sa, epi, slot, COUT, tid, th, idx, s);
-    fence_before_thread_sync();
     __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = tmem_base_s;
-    constexpr uint32_t IDESC2 = idesc_tf32(128, 2 * COUT), IDESC1 = idesc_tf32(128, COUT);
 
-    if (warp == STAGE_WARPS) {
-        // ============ MMA warp: converged loop, descriptors in uniform registers, one elected lane issues ============
+    if (warp >= STAGE_WARPS) {
+        // ============ MMA warpgroups: warpgroup w owns the m64 tiles w*MTC .. w*MTC+MTC-1 of the CTA's rows ============
+        const int w = (warp - STAGE_WARPS) >> 2, wq = warp & 3;
         const uint32_t s0 = smem_u32(smem);
-        const uint64_t dA0 = smem_desc(s0, Cfg::A_PLANE, 128);
-        const uint64_t dB0 = smem_desc(s0 + Cfg::A_PLANES * Cfg::A_BYTES, Cfg::B_PLANE, 128);
+        // A_hi*B_hi and the two cross terms in separate register blocks (a wgmma into a sub-block of another wgmma's
+        // accumulators leaves ptxas without registers for the pipeline and serialises every wgmma)
+        float acc[MTC][Cfg::ACC], cor[MTC][Cfg::ACC];
+#pragma unroll
+        for (int j = 0; j < MTC; ++j)
+#pragma unroll
+            for (int x = 0; x < Cfg::ACC; ++x) acc[j][x] = cor[j][x] = 0.0f;
         for (int c = 0; c < Cfg::NCHUNK; ++c) {
             const int st = c % NST;
             mbar_wait(&full_bar[st], (c / NST) & 1);             // the staging group has filled (and fenced) this stage
-            fence_after_thread_sync();
-            TRACE(lane == 0, 16 + 2 * c);
-            const uint64_t so = (uint64_t)((st * Cfg::STAGE_BYTES) >> 4);    // descriptor address field is in 16-byte units
-            if (elect_one()) {
+            const uint32_t sa0 = s0 + st * Cfg::STAGE_BYTES, sb0 = sa0 + Cfg::A_PLANES * Cfg::A_BYTES;
+            wgmma_fence();
 #pragma unroll
-                for (int mt = 0; mt < MTC; ++mt) {
-                    const uint32_t d = tmem_base + mt * 2 * COUT;
+            for (int k8 = 0; k8 < KC / 8; ++k8) {
+                const uint64_t dB = smem_desc(sb0 + 2 * k8 * Cfg::B_PLANE, Cfg::B_PLANE, 128);
 #pragma unroll
-                    for (int k8 = 0; k8 < KC / 8; ++k8) {
-                        const uint64_t dAh = dA0 + so + (uint64_t)((2 * k8 * Cfg::A_PLANE + mt * 128 * 16) >> 4);
-                        const uint64_t dB = dB0 + so + (uint64_t)((2 * k8 * Cfg::B_PLANE) >> 4);
-                        mma_tf32(d, dAh, dB, IDESC2, (c | k8) != 0);                                  // A_hi * [B_hi ; B_lo]
-                        if (!IN_U8) mma_tf32(d, dAh + (uint64_t)(Cfg::A_BYTES >> 4), dB, IDESC1, 1);  // A_lo * B_hi
+                for (int j = 0; j < MTC; ++j) {
+                    const uint64_t dAh = smem_desc(sa0 + 2 * k8 * Cfg::A_PLANE + (w * MTC + j) * 1024, Cfg::A_PLANE, 128);
+                    wgmma_tf32<COUT>(acc[j], dAh, dB, 1);                                                      // A_hi * B_hi
+                    wgmma_tf32<COUT>(cor[j], dAh, dB + (uint64_t)((COUT * 16) >> 4), 1);                       // A_hi * B_lo
+                    if (!IN_U8) wgmma_tf32<COUT>(cor[j], dAh + (uint64_t)(Cfg::A_BYTES >> 4), dB, 1);          // A_lo * B_hi
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                                     // the previous chunk's MMAs have read their stage
+            __syncwarp();
+            if (c > 0 && lane == 0) mbar_arrive(&empty_bar[(c - 1) % NST]);
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int j = 0; j < MTC; ++j) {
+            fence_regs<Cfg::ACC>(acc[j]);
+            fence_regs<Cfg::ACC>(cor[j]);
+        }
+        // ---- epilogue: registers -> (/255) + bias (+BN) + activation -> NHWC global ----
+        float* out = out_base + slot * out_slot_stride + img * out_img_stride;
+        constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
+#pragma unroll
+        for (int j = 0; j < MTC; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = row0 + (w * MTC + j) * 64 + wq * 16 + (lane >> 2) + 8 * h;
+                if (m < Cfg::M) {
+#pragma unroll
+                    for (int i = 0; i < COUT / 8; ++i) {
+                        const int n = 8 * i + 2 * (lane & 3);
+                        float v0 = acc[j][4 * i + 2 * h] + cor[j][4 * i + 2 * h];
+                        float v1 = acc[j][4 * i + 2 * h + 1] + cor[j][4 * i + 2 * h + 1];
+                        if (IN_U8) { v0 *= IN_SCALE; v1 *= IN_SCALE; }
+                        *reinterpret_cast<float2*>(out + (int64_t)m * COUT + n) = make_float2(epi_s[n].apply(v0), epi_s[n + 1].apply(v1));
                     }
                 }
-                mma_commit(&empty_bar[st]);                      // stage reusable once these MMAs have read it
-                if (c == Cfg::NCHUNK - 1) mma_commit(&done_bar); // every MMA of the tile has completed
             }
-            __syncwarp();
-            TRACE(lane == 0, 17 + 2 * c);
-        }
     } else {
         // ============== staging groups: perturb + im2col -> shared memory (group g <-> stage g) ==============
         const int g = warp >> 2, wg = warp & 3, tg = tid & 127;
@@ -188,7 +194,6 @@ conv_tc_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict_
 
         for (int c = g, it = 0; c < Cfg::NCHUNK; c += TC_GROUPS, ++it) {
             // ---- raw global loads of the chunk (issued before the stage wait so that their latency overlaps it) ----
-            TRACE(tg == 0, 128 + (g * 16 + it) * 4 + 0);
             const int k = c * KC + 4 * q;
             const int ci = k % CIN, t = k / CIN;
             const int ky = t / KS, kx = t - ky * KS;
@@ -215,7 +220,6 @@ conv_tc_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict_
                 }
             }
             mbar_wait(&empty_bar[g], (it & 1) ^ 1);              // the MMAs of this group's previous chunk have drained the stage
-            TRACE(tg == 0, 128 + (g * 16 + it) * 4 + 1);
             // ---- convert + store: A ----
 #pragma unroll
             for (int i = 0; i < PASSES; ++i) {
@@ -234,7 +238,6 @@ conv_tc_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict_
                     sts128(sA_lo + i * 512, lo);
                 }
             }
-            TRACE(tg == 0, 128 + (g * 16 + it) * 4 + 2);
             // ---- perturb + convert + store: B ----
 #pragma unroll
             for (int i = 0; i < BPT; ++i) {
@@ -252,45 +255,8 @@ conv_tc_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict_
             fence_proxy_async_smem();                            // generic-proxy writes -> async proxy
             __syncwarp();
             if (lane == 0) mbar_arrive(&full_bar[g]);
-            TRACE(tg == 0, 128 + (g * 16 + it) * 4 + 3);
-        }
-        // ---- epilogue: TMEM -> registers -> (/255) + bias (+BN) + activation -> NHWC global ----
-        mbar_wait(&done_bar, 0);
-        fence_after_thread_sync();
-        TRACE(tid == 0, 2);
-        float* out = out_base + slot * out_slot_stride + img * out_img_stride;
-        // warp w may only touch TMEM lanes 32*(w%4)..+31; the (M-tile, 16-column group) work items are dealt round-robin
-        // to the TC_GROUPS warps that share a lane group
-        constexpr int NJ = COUT / 16;
-        constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
-#pragma unroll
-        for (int p = 0; p < MTC * NJ; ++p) {
-            if (p % TC_GROUPS != g) continue;
-            const int mt = p / NJ, n0 = (p % NJ) * 16;
-            float v[16], v2[16];
-            tmem_ld16(tmem_base + ((uint32_t)(wg * 32) << 16) + (uint32_t)(mt * 2 * COUT + n0), v);
-            tmem_ld16(tmem_base + ((uint32_t)(wg * 32) << 16) + (uint32_t)(mt * 2 * COUT + COUT + n0), v2);
-#pragma unroll
-            for (int x = 0; x < 16; ++x) v[x] += v2[x];
-            const int m = row0 + mt * 128 + wg * 32 + lane;
-            if (m < Cfg::M) {
-                float4* dst = reinterpret_cast<float4*>(out + (int64_t)m * COUT + n0);
-#pragma unroll
-                for (int x = 0; x < 16; x += 4) {
-                    if (IN_U8) { v[x] *= IN_SCALE; v[x + 1] *= IN_SCALE; v[x + 2] *= IN_SCALE; v[x + 3] *= IN_SCALE; }
-                    dst[x / 4] = make_float4(epi_s[n0 + x].apply(v[x]), epi_s[n0 + x + 1].apply(v[x + 1]),
-                                             epi_s[n0 + x + 2].apply(v[x + 2]), epi_s[n0 + x + 3].apply(v[x + 3]));
-                }
-            }
         }
     }
-    fence_before_thread_sync();
-    __syncthreads();
-    TRACE(tid == 0, 3);
-#ifdef DNE_CONV_TRACE
-    if (TRACE_ON && tid == 0) { unsigned long long ns; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(ns)); g_conv_trace[5] = (long long)ns; }
-#endif
-    if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 // =====================================================================================================
@@ -339,37 +305,63 @@ int dne_launch_conv_layer_tc(const SlotArgs& sa, const dne_layer_desc& L, const 
 // =====================================================================================================
 // Dense layer, shared-theta part on the tensor cores:  part[split][m][n] = sum_{k in split} X[m][k] * W[k][n]
 // (same contract as dense_theta_gemm_kernel).  CTA tile 128 x 128, k-chunks of 16, 3xTF32, operands staged by the
-// threads (A rows are K-contiguous float4 loads; B is transposed to [n][k] quads on the fly), two smem stages.
+// threads (A rows are K-contiguous float4 loads; B is transposed to [n][k] quads on the fly), three smem stages.  The
+// two warpgroups stage together and each issues the wgmmas of one m64 half of the tile: a stage is rewritten three
+// chunks after it was read, by which time every warpgroup has waited for those wgmmas (wgmma_wait<1>) and passed a
+// block barrier since -- one __syncthreads per chunk.
 // =====================================================================================================
-constexpr int TG_BM = 128, TG_BN = 128, TG_KC = 16;
+constexpr int TG_BM = 128, TG_BN = 128, TG_KC = 16, TG_NST = 3;
 constexpr int TG_A_PLANE = TG_BM * 16, TG_B_PLANE = TG_BN * 16;
 constexpr int TG_A_BYTES = (TG_KC / 4) * TG_A_PLANE, TG_B_BYTES = (TG_KC / 4) * TG_B_PLANE;
 constexpr int TG_STAGE_BYTES = 2 * TG_A_BYTES + 2 * TG_B_BYTES;
-constexpr int TG_SMEM_BYTES = 2 * TG_STAGE_BYTES + 128;
+constexpr int TG_SMEM_BYTES = TG_NST * TG_STAGE_BYTES + 128;
 
-__global__ void __launch_bounds__(TG_THREADS)
+// stage chunk (rawA, rawB) into stage st, split hi / lo
+__device__ __forceinline__ void tg_stage(uint32_t s0, int st, int tid, const float4 (&rawA)[2], const float (&rawB)[2][4]) {
+    const uint32_t sA_hi = s0 + st * TG_STAGE_BYTES, sA_lo = sA_hi + TG_A_BYTES, sB_hi = sA_lo + TG_A_BYTES, sB_lo = sB_hi + TG_B_BYTES;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int u = tid + i * TG_THREADS;
+        float4 hi, lo;
+        split_tf32_fast(rawA[i].x, hi.x, lo.x);
+        split_tf32_fast(rawA[i].y, hi.y, lo.y);
+        split_tf32_fast(rawA[i].z, hi.z, lo.z);
+        split_tf32_fast(rawA[i].w, hi.w, lo.w);
+        sts128(sA_hi + u * 16, hi);                              // (u / TG_BM) * TG_A_PLANE + (u % TG_BM) * 16 == u * 16
+        sts128(sA_lo + u * 16, lo);
+        split_tf32_fast(rawB[i][0], hi.x, lo.x);
+        split_tf32_fast(rawB[i][1], hi.y, lo.y);
+        split_tf32_fast(rawB[i][2], hi.z, lo.z);
+        split_tf32_fast(rawB[i][3], hi.w, lo.w);
+        sts128(sB_hi + u * 16, hi);
+        sts128(sB_lo + u * 16, lo);
+    }
+}
+// this warpgroup's m64 half of the 128 x 128 tile: A_hi*B_hi + A_lo*B_hi + A_hi*B_lo over one chunk
+__device__ __forceinline__ void tg_mma(uint32_t s0, int st, int half, float (&acc)[64], bool overwrite) {
+    const uint32_t sA = s0 + st * TG_STAGE_BYTES + half * 1024, sB = s0 + st * TG_STAGE_BYTES + 2 * TG_A_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k8 = 0; k8 < TG_KC / 8; ++k8) {
+        const uint64_t dAh = smem_desc(sA + 2 * k8 * TG_A_PLANE, TG_A_PLANE, 128), dBh = smem_desc(sB + 2 * k8 * TG_B_PLANE, TG_B_PLANE, 128);
+        wgmma_tf32<128>(acc, dAh, dBh, !(overwrite && k8 == 0));
+        wgmma_tf32<128>(acc, dAh + (uint64_t)(TG_A_BYTES >> 4), dBh, 1);
+        wgmma_tf32<128>(acc, dAh, dBh + (uint64_t)(TG_B_BYTES >> 4), 1);
+    }
+    wgmma_commit();
+}
+
+__global__ void __launch_bounds__(TG_THREADS, 1)
 theta_gemm_tc_kernel(const float* __restrict__ X, int M, int K, int N, const float* __restrict__ W, int k_per_split,
                      float* __restrict__ part) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
-    __shared__ uint64_t bars[2];
-    __shared__ uint32_t tmem_base_s;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int half = warp >> 2, wq = warp & 3;
     const int m0 = blockIdx.y * TG_BM, n0 = blockIdx.x * TG_BN, split = blockIdx.z;
     const int kbeg = split * k_per_split, kend = min(K, kbeg + k_per_split);
     const int nchunk = (kend - kbeg + TG_KC - 1) / TG_KC;
-
-    if (warp == 0) tmem_alloc(&tmem_base_s, 128);
-    if (tid == 32) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
-        fence_mbar_init();
-    }
-    fence_before_thread_sync();
-    __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = tmem_base_s;
-    constexpr uint32_t IDESC = idesc_tf32(128, TG_BN);
+    const uint32_t s0 = smem_u32(smem);
 
     // A: 128 rows x 4 k-quads = 512 units; B: 128 n x 4 k-quads = 512 units -> 2 + 2 units per thread
     float4 rawA[2];
@@ -388,77 +380,33 @@ theta_gemm_tc_kernel(const float* __restrict__ X, int M, int K, int N, const flo
             for (int j = 0; j < 4; ++j) rawB[i][j] = (n < N && kb + j < kend) ? W[(int64_t)(kb + j) * N + n] : 0.0f;
         }
     };
+    float acc[64];
+#pragma unroll
+    for (int x = 0; x < 64; ++x) acc[x] = 0.0f;
     if (nchunk > 0) load_chunk(0);
     for (int c = 0; c < nchunk; ++c) {
-        const int st = c & 1;
-        if (c >= 2) mbar_wait(&bars[st], ((c >> 1) - 1) & 1);
-        const uint32_t sA_hi = smem_u32(smem) + st * TG_STAGE_BYTES, sA_lo = sA_hi + TG_A_BYTES, sB_hi = sA_lo + TG_A_BYTES,
-                       sB_lo = sB_hi + TG_B_BYTES;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int u = tid + i * TG_THREADS;
-            float4 hi, lo;
-            split_tf32_fast(rawA[i].x, hi.x, lo.x);
-            split_tf32_fast(rawA[i].y, hi.y, lo.y);
-            split_tf32_fast(rawA[i].z, hi.z, lo.z);
-            split_tf32_fast(rawA[i].w, hi.w, lo.w);
-            sts128(sA_hi + u * 16, hi);                          // (u / TG_BM) * TG_A_PLANE + (u % TG_BM) * 16 == u * 16
-            sts128(sA_lo + u * 16, lo);
-            split_tf32_fast(rawB[i][0], hi.x, lo.x);
-            split_tf32_fast(rawB[i][1], hi.y, lo.y);
-            split_tf32_fast(rawB[i][2], hi.z, lo.z);
-            split_tf32_fast(rawB[i][3], hi.w, lo.w);
-            sts128(sB_hi + u * 16, hi);
-            sts128(sB_lo + u * 16, lo);
-        }
+        const int st = c % TG_NST;
+        tg_stage(s0, st, tid, rawA, rawB);
         if (c + 1 < nchunk) load_chunk(c + 1);
         fence_proxy_async_smem();
         __syncthreads();
-        if (warp == 0) {                                         // converged warp, one elected lane issues (tc05.cuh: elect_one)
-            fence_after_thread_sync();
-            const uint64_t dA = smem_desc(smem_u32(smem) + st * TG_STAGE_BYTES, TG_A_PLANE, 128);
-            const uint64_t dB = smem_desc(smem_u32(smem) + st * TG_STAGE_BYTES + 2 * TG_A_BYTES, TG_B_PLANE, 128);
-            if (elect_one()) {
-#pragma unroll
-                for (int k8 = 0; k8 < TG_KC / 8; ++k8) {
-                    const uint64_t dAh = dA + (uint64_t)((2 * k8 * TG_A_PLANE) >> 4), dBh = dB + (uint64_t)((2 * k8 * TG_B_PLANE) >> 4);
-                    mma_tf32(tmem_base, dAh, dBh, IDESC, (c | k8) != 0);
-                    mma_tf32(tmem_base, dAh + (uint64_t)(TG_A_BYTES >> 4), dBh, IDESC, 1);
-                    mma_tf32(tmem_base, dAh, dBh + (uint64_t)(TG_B_BYTES >> 4), IDESC, 1);
-                }
-                mma_commit(&bars[st]);
-            }
-            __syncwarp();
-        }
+        tg_mma(s0, st, half, acc, false);                    // acc starts at zero: no non-wgmma write inside the pipeline
+        wgmma_wait<1>();
     }
-    if (nchunk > 0) mbar_wait(&bars[(nchunk - 1) & 1], ((nchunk - 1) >> 1) & 1);
-    fence_after_thread_sync();
+    wgmma_wait<0>();
+    fence_regs<64>(acc);
     float* P = part + (int64_t)split * M * N;
-    const int lg = warp & 3, ch = warp >> 2;
-    const int m = m0 + lg * 32 + lane;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int nc = ch * 64 + j * 16;
-        float v[16];
-        if (nchunk > 0) tmem_ld16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)nc, v);
-        else {
-#pragma unroll
-            for (int x = 0; x < 16; ++x) v[x] = 0.0f;
-        }
+    for (int h = 0; h < 2; ++h) {
+        const int m = m0 + half * 64 + wq * 16 + (lane >> 2) + 8 * h;
         if (m < M) {
 #pragma unroll
-            for (int x = 0; x < 16; x += 4) {
-                const int n = n0 + nc + x;
-                if (n + 3 < N) *reinterpret_cast<float4*>(P + (int64_t)m * N + n) = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
-                else
-                    for (int y = 0; y < 4; ++y)
-                        if (n + y < N) P[(int64_t)m * N + n + y] = v[x + y];
+            for (int j = 0; j < 16; ++j) {
+                const int n = n0 + 8 * j + 2 * (lane & 3);         // N % 4 == 0: n < N implies n + 1 < N
+                if (n < N) *reinterpret_cast<float2*>(P + (int64_t)m * N + n) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
             }
         }
     }
-    fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, 128);
 }
 
 // returns 0 on launch, DNE_ERR_UNSUP if the shape is not covered (caller falls back to the SIMT GEMM)
@@ -484,19 +432,18 @@ int dne_launch_theta_gemm_tc(const float* X, int M, int K, int N, const float* W
 // Per-member dense layer of the virtual-batch-norm reference pass on the tensor cores (policies.py:322-328,399; the fc
 // of ESAtariPolicy / ModelVirtualBN): out[slot][m][n] = sum_k X[slot][m][k] * fl(theta_w + fl(s*noise))[k][n] + bias_n
 // for the M = n_ref reference rows of every member.  Same tile engine as theta_gemm_tc_kernel (CTA tile 128 x 128,
-// 3xTF32, thread-staged operands, two smem stages) with blockIdx.z = member: the B operand is the member's PERTURBED
+// 3xTF32, thread-staged operands, three smem stages) with blockIdx.z = member: the B operand is the member's PERTURBED
 // weight matrix, formed from the theta rows and the member's noise rows while staging; the whole K range in one CTA.
 // =====================================================================================================
-__global__ void __launch_bounds__(TG_THREADS, 2)
+__global__ void __launch_bounds__(TG_THREADS, 1)
 member_gemm_tc_kernel(SlotArgs sa, int64_t off_w, int64_t off_b, const float* __restrict__ X, int64_t x_slot_stride, int M,
                       int K, int N, float* __restrict__ out, int64_t out_slot_stride) {
     const int slot = blockIdx.z;
     if (!slot_active(sa, slot)) return;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
-    __shared__ uint64_t bars[2];
-    __shared__ uint32_t tmem_base_s;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int half = warp >> 2, wq = warp & 3;
     const int m0 = blockIdx.y * TG_BM, n0 = blockIdx.x * TG_BN;
     const int nchunk = (K + TG_KC - 1) / TG_KC;
     const float* th = slot_theta(sa, slot);
@@ -505,22 +452,10 @@ member_gemm_tc_kernel(SlotArgs sa, int64_t off_w, int64_t off_b, const float* __
     const float* tw = th + off_w;
     const float* nz = sa.noise + idx + off_w;
     const float* x = X + (int64_t)slot * x_slot_stride;
-
-    if (warp == 0) tmem_alloc(&tmem_base_s, 128);
-    if (tid == 32) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
-        fence_mbar_init();
-    }
-    fence_before_thread_sync();
-    __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = tmem_base_s;
-    constexpr uint32_t IDESC = idesc_tf32(128, TG_BN);
+    const uint32_t s0 = smem_u32(smem);
 
     constexpr int MG_DRAIN = 16;
-    const int lg = warp & 3, ch = warp >> 2;                     // epilogue / drain map: TMEM lane quarter, 64-column half
-    float accr[64];
+    float acc[64], accr[64];
 #pragma unroll
     for (int xx = 0; xx < 64; ++xx) accr[xx] = 0.0f;
     float4 rawA[2];
@@ -543,89 +478,37 @@ member_gemm_tc_kernel(SlotArgs sa, int64_t off_w, int64_t off_b, const float* __
     };
     load_chunk(0);
     for (int c = 0; c < nchunk; ++c) {
-        const int st = c & 1;
-        if (c >= 2) mbar_wait(&bars[st], ((c >> 1) - 1) & 1);
-        const uint32_t sA_hi = smem_u32(smem) + st * TG_STAGE_BYTES, sA_lo = sA_hi + TG_A_BYTES, sB_hi = sA_lo + TG_A_BYTES,
-                       sB_lo = sB_hi + TG_B_BYTES;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int u = tid + i * TG_THREADS;
-            float4 hi, lo;
-            split_tf32_fast(rawA[i].x, hi.x, lo.x);
-            split_tf32_fast(rawA[i].y, hi.y, lo.y);
-            split_tf32_fast(rawA[i].z, hi.z, lo.z);
-            split_tf32_fast(rawA[i].w, hi.w, lo.w);
-            sts128(sA_hi + u * 16, hi);
-            sts128(sA_lo + u * 16, lo);
-            split_tf32_fast(rawB[i][0], hi.x, lo.x);
-            split_tf32_fast(rawB[i][1], hi.y, lo.y);
-            split_tf32_fast(rawB[i][2], hi.z, lo.z);
-            split_tf32_fast(rawB[i][3], hi.w, lo.w);
-            sts128(sB_hi + u * 16, hi);
-            sts128(sB_lo + u * 16, lo);
-        }
+        const int st = c % TG_NST;
+        tg_stage(s0, st, tid, rawA, rawB);
         if (c + 1 < nchunk) load_chunk(c + 1);
         fence_proxy_async_smem();
         __syncthreads();
-        if (warp == 0) {
-            fence_after_thread_sync();
-            const uint64_t dA = smem_desc(smem_u32(smem) + st * TG_STAGE_BYTES, TG_A_PLANE, 128);
-            const uint64_t dB = smem_desc(smem_u32(smem) + st * TG_STAGE_BYTES + 2 * TG_A_BYTES, TG_B_PLANE, 128);
-            if (elect_one()) {
-#pragma unroll
-                for (int k8 = 0; k8 < TG_KC / 8; ++k8) {
-                    const uint64_t dAh = dA + (uint64_t)((2 * k8 * TG_A_PLANE) >> 4), dBh = dB + (uint64_t)((2 * k8 * TG_B_PLANE) >> 4);
-                    mma_tf32(tmem_base, dAh, dBh, IDESC, ((c % MG_DRAIN) | k8) != 0);
-                    mma_tf32(tmem_base, dAh + (uint64_t)(TG_A_BYTES >> 4), dBh, IDESC, 1);
-                    mma_tf32(tmem_base, dAh, dBh + (uint64_t)(TG_B_BYTES >> 4), IDESC, 1);
-                }
-                mma_commit(&bars[st]);
-            }
-            __syncwarp();
-        }
+        tg_mma(s0, st, half, acc, (c % MG_DRAIN) == 0);
         if ((c % MG_DRAIN) == MG_DRAIN - 1 || c == nchunk - 1) {
-            // drain the TMEM accumulator into fp32 registers every MG_DRAIN chunks (K = 256): the tensor core's accumulator add
-            // is not round-to-nearest, and over K = 3872 its bias reached 4e-5 (VBN statistics are compared at 2e-5)
-            mbar_wait(&bars[st], (c >> 1) & 1);                  // every MMA up to chunk c has completed
-            fence_after_thread_sync();
+            // fold the tensor-core accumulator into fp32 registers every MG_DRAIN chunks (K = 256): the tensor core's
+            // accumulator add is not round-to-nearest, and over K = 3872 its bias reached 4e-5 (VBN statistics are compared
+            // at 2e-5)
+            wgmma_wait<0>();
+            fence_regs<64>(acc);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                float v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(ch * 64 + j * 16), v);
-#pragma unroll
-                for (int xx = 0; xx < 16; ++xx) accr[j * 16 + xx] += v[xx];
-            }
-            fence_before_thread_sync();                          // ordered before the next chunk's __syncthreads + MMA (accumulate = 0)
+            for (int xx = 0; xx < 64; ++xx) accr[xx] += acc[xx];
+        } else {
+            wgmma_wait<1>();
         }
     }
     float* o = out + (int64_t)slot * out_slot_stride;
-    const int m = m0 + lg * 32 + lane;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int nc = ch * 64 + j * 16;
-        float v[16];
+    for (int j = 0; j < 16; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);               // N % 4 == 0: n < N implies n + 1 < N
+        if (n >= N) continue;
+        const float b0 = off_b >= 0 ? perturbed(th[off_b + n], s, sa.noise[idx + off_b + n]) : 0.0f;
+        const float b1 = off_b >= 0 ? perturbed(th[off_b + n + 1], s, sa.noise[idx + off_b + n + 1]) : 0.0f;
 #pragma unroll
-        for (int xx = 0; xx < 16; ++xx) v[xx] = accr[j * 16 + xx];
-#pragma unroll
-        for (int xx = 0; xx < 16; ++xx) {
-            const int n = n0 + nc + xx;
-            const float bias = (off_b >= 0 && n < N) ? perturbed(th[off_b + n], s, sa.noise[idx + off_b + n]) : 0.0f;
-            v[xx] += bias;
-        }
-        if (m < M) {
-#pragma unroll
-            for (int xx = 0; xx < 16; xx += 4) {
-                const int n = n0 + nc + xx;
-                if (n + 3 < N) *reinterpret_cast<float4*>(o + (int64_t)m * N + n) = make_float4(v[xx], v[xx + 1], v[xx + 2], v[xx + 3]);
-                else
-                    for (int y = 0; y < 4; ++y)
-                        if (n + y < N) o[(int64_t)m * N + n + y] = v[xx + y];
-            }
+        for (int h = 0; h < 2; ++h) {
+            const int m = m0 + half * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            if (m < M) *reinterpret_cast<float2*>(o + (int64_t)m * N + n) = make_float2(accr[4 * j + 2 * h] + b0, accr[4 * j + 2 * h + 1] + b1);
         }
     }
-    fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, 128);
 }
 
 // returns 0 on launch, DNE_ERR_UNSUP if the shape is not covered (caller falls back to the SIMT member GEMM)

@@ -1,38 +1,37 @@
-// theta_gemm_tma.cu -- the shared-theta part of a dense layer, X[slots,K] . theta_w[K,N], as a pure TMA + tcgen05 kernel.
+// theta_gemm_tma.cu -- the shared-theta part of a dense layer, X[slots,K] . theta_w[K,N], as a pure TMA + wgmma kernel.
 //
 //   part[split][m][n] = sum_{k in split} X[m][k] * W[k][n]          (same contract as theta_gemm_tc_kernel / dense_theta_gemm_kernel)
 //
-// The r01 kernel (tc_conv.cu: theta_gemm_tc_kernel, 31 us per 256-slot LargeModel tick) staged both operands through the
-// threads (global -> registers -> TF32 split -> st.shared) with two stages and a block barrier per 16-wide chunk.  Here
-// both operands already exist in global memory in the UMMA K-major canonical layout, as 2 x fp16 splits (tc05.cuh:
-// x = h0 + h1*2^-11; kind::f16 runs at twice the MAC rate of kind::tf32 and the operands are half the bytes):
+// theta_gemm_tc_kernel (tc_conv.cu) stages both operands through the threads (global -> registers -> TF32 split ->
+// st.shared) with a block barrier per 16-wide chunk.  Here both operands already exist in global memory in the wgmma
+// K-major canonical layout, as 2 x fp16 splits (wgmma.cuh: x = h0 + h1*2^-11; f16 wgmma runs at twice the MAC rate of
+// tf32 and the operands are half the bytes):
 //   * W changes once per generation: dne_theta_prepare() relays it out (theta_prep_kernel) into
 //       Wc[n tile of 128][k octet][h0 | h1][128 n][8 k]     one k-octet plane = [B_h0 ; B_h1] stacked along N = 4 KB
 //   * X is the output of the last convolution: its epilogue (conv_s2d.cu) writes, besides the NHWC vector the noise GEMV
 //     streams, the same values as
 //       Xc[m tile of 128][k octet][h0 | h1][128 slots][8 k] one k-octet plane = [A_h0 ; A_h1] = 4 KB
 // so a K chunk of 32 of either operand is one contiguous 16 KB run and the whole main loop is: one producer thread issuing
-// cp.async.bulk into a 4-stage ring, one MMA thread issuing tcgen05.mma (A_h0*[B_h0;B_h1] as one N = 256 MMA into
-// [main | correction] accumulator columns plus A_h1*B_h0 into the correction columns; result = main + 2^-11 * correction),
-// no staging threads at all.  A CTA owns BOTH 128-row M tiles of a 128-column N tile (the B chunk is read
-// once for 256 slots; 2 x 256 accumulator columns = the whole TMEM) and one K split; partials are deterministic.
-// The N tiles of one K split form a thread-block cluster: every CTA fetches 1/CL of the shared A chunk and MULTICASTS it
-// into all CL CTAs' stages (cp.async.bulk ... .multicast::cluster), so X crosses the L2 -> SM fabric once per split instead
-// of once per N tile; a stage is recycled when the MMAs of ALL CL CTAs have read it (tcgen05.commit multicast on the
-// empty barriers).
+// cp.async.bulk into a 4-stage ring and two MMA warpgroups, each issuing A_h0*[B_h0;B_h1] as one N = 256 wgmma into its
+// [main | correction] accumulator registers plus A_h1*B_h0 into the correction half (result = main + 2^-11 * correction)
+// for one m64 half of the CTA's 128 x 128 tile; no staging threads at all.  A CTA owns one M tile, one N tile and one K
+// split; partials are deterministic.
+// Optionally (dne_set_option("theta_mc", 1)) the N tiles of one K split form a thread-block cluster: every CTA fetches
+// 1/CL of the shared A chunk and MULTICASTS it into all CL CTAs' stages (cp.async.bulk ... .multicast::cluster), so X
+// crosses the L2 -> SM fabric once per split instead of once per N tile; a stage is recycled when the MMA warps of ALL CL
+// CTAs have read it (remote mbarrier arrivals on every peer's empty barrier).
 #include "common.cuh"
 #include "forward.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
-using namespace tc05;
+using namespace wg;
 
 int g_dne_theta_mc = 0;
 namespace {
 constexpr int TGM_KC = 32, TGM_STAGES = 4;                 // 32 k = four k-octet planes per chunk
 constexpr int TGM_PLANE = 256 * 16;                         // bytes of one k-quad plane: 128 hi rows + 128 lo rows
 constexpr int TGM_CHUNK = (TGM_KC / 8) * TGM_PLANE;         // 16 KB per operand tile and chunk
-constexpr int TGM_EPI_WARPS = 8;
-constexpr int TGM_THREADS = 32 * (2 + TGM_EPI_WARPS);
+constexpr int TGM_THREADS = 32 * 9;                         // two MMA warpgroups + one TMA producer warp
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -50,47 +49,40 @@ __device__ __forceinline__ void bulk_g2s_mc(void* smem_dst, const void* gmem_src
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
                  : "memory");
 }
-__device__ __forceinline__ void mma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 
-template <int MT, int CL>
+template <int CL>
 __global__ void __launch_bounds__(TGM_THREADS, 1)
 theta_gemm_tma_kernel(const float* __restrict__ Xc, const float* __restrict__ Wc, int M, int N, int KQ, int chunks_per_split,
                       int n_chunks, float* __restrict__ part) {
-    constexpr int STAGE = (MT + 1) * TGM_CHUNK;
+    constexpr int STAGE = 2 * TGM_CHUNK;                    // [A chunk of the M tile | B chunk of the N tile]
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
-    __shared__ uint64_t full_bar[TGM_STAGES], empty_bar[TGM_STAGES], done_bar;
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full_bar[TGM_STAGES], empty_bar[TGM_STAGES];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ntile = blockIdx.x, split = blockIdx.y, mgroup = blockIdx.z;
+    const int ntile = blockIdx.x, split = blockIdx.y, mtile = blockIdx.z;
     const int c0 = split * chunks_per_split, c1 = min(n_chunks, c0 + chunks_per_split);
     const int nc = max(0, c1 - c0);
-    constexpr int TCOLS = MT * 256;
 
     pdl_trigger();                                          // common.cuh: PDL chain of the tick
-    if (warp == 0) tmem_alloc(&tmem_base_s, TCOLS);
-    if (tid == 32) {
-        for (int i = 0; i < TGM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CL); }
-        mbar_init(&done_bar, 1);
+    if (tid == 0) {
+        for (int i = 0; i < TGM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8 * CL); }
         fence_mbar_init();
     }
-    fence_before_thread_sync();
     __syncthreads();
-    fence_after_thread_sync();
     if (CL > 1) cluster_sync_all();                         // every peer's barriers exist before anyone multicasts into it
-    const uint32_t tmem_base = tmem_base_s;
     constexpr uint16_t CL_MASK = (uint16_t)((1u << CL) - 1);
     pdl_wait();                                             // Xc is written by the previous kernel (conv3 epilogue); part is read by the next
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===== TMA producer =====
         if (lane == 0) {
-            const uint8_t* xa = (const uint8_t*)Xc + (size_t)(mgroup * MT) * KQ * TGM_PLANE;
+            const uint8_t* xa = (const uint8_t*)Xc + (size_t)mtile * KQ * TGM_PLANE;
             const uint8_t* wb = (const uint8_t*)Wc + (size_t)ntile * KQ * TGM_PLANE;
             for (int i = 0; i < nc; ++i) {
                 const int st = i % TGM_STAGES;
@@ -99,87 +91,68 @@ theta_gemm_tma_kernel(const float* __restrict__ Xc, const float* __restrict__ Wc
                 const size_t koff = (size_t)(c0 + i) * TGM_CHUNK;
                 uint8_t* dst = smem + st * STAGE;
                 if (CL == 1) {
-#pragma unroll
-                    for (int mt = 0; mt < MT; ++mt)
-                        bulk_g2s(dst + mt * TGM_CHUNK, xa + (size_t)mt * KQ * TGM_PLANE + koff, TGM_CHUNK, &full_bar[st]);
+                    bulk_g2s(dst, xa + koff, TGM_CHUNK, &full_bar[st]);
                 } else {
-                    // this CTA's 1/CL slice of the A region of the stage, delivered to every CTA of the cluster
-                    constexpr int SLICE = MT * TGM_CHUNK / CL;
-                    const int off = (int)cluster_ctarank() * SLICE, mt = off / TGM_CHUNK, in_chunk = off % TGM_CHUNK;
-                    bulk_g2s_mc(dst + off, xa + (size_t)mt * KQ * TGM_PLANE + koff + in_chunk, SLICE, &full_bar[st], CL_MASK);
+                    // this CTA's 1/CL slice of the A chunk, delivered to every CTA of the cluster
+                    constexpr int SLICE = TGM_CHUNK / CL;
+                    const int off = (int)cluster_ctarank() * SLICE;
+                    bulk_g2s_mc(dst + off, xa + koff + off, SLICE, &full_bar[st], CL_MASK);
                 }
-                bulk_g2s(dst + MT * TGM_CHUNK, wb + koff, TGM_CHUNK, &full_bar[st]);
+                bulk_g2s(dst + TGM_CHUNK, wb + koff, TGM_CHUNK, &full_bar[st]);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (converged warp, one elected lane) =====
-        constexpr uint32_t IDESC2 = idesc_f16(128, 256), IDESC1 = idesc_f16(128, 128);
-        const uint64_t d0 = smem_desc(smem_u32(smem), TGM_PLANE, 128);
+    } else {
+        // ===== MMA warpgroups: warpgroup w owns rows 64*w .. 64*w+63 of the M tile =====
+        const int w = warp >> 2, wq = warp & 3;
+        // main and correction accumulators in separate register blocks (a wgmma into a sub-block of another wgmma's
+        // accumulators leaves ptxas without registers for the pipeline and serialises every wgmma)
+        float acc[64], cor[64];
+#pragma unroll
+        for (int x = 0; x < 64; ++x) acc[x] = cor[x] = 0.0f;
+        const uint32_t s0 = smem_u32(smem);
         for (int i = 0; i < nc; ++i) {
             const int st = i % TGM_STAGES;
             mbar_wait(&full_bar[st], (i / TGM_STAGES) & 1);
-            fence_after_thread_sync();
-            if (elect_one()) {
-                const uint64_t ds = d0 + (uint64_t)((st * STAGE) >> 4);
+            wgmma_fence();
 #pragma unroll
-                for (int k16 = 0; k16 < TGM_KC / 16; ++k16) {
-                    const uint64_t dB = ds + (uint64_t)((MT * TGM_CHUNK + 2 * k16 * TGM_PLANE) >> 4);
-#pragma unroll
-                    for (int mt = 0; mt < MT; ++mt) {
-                        const uint64_t dAh = ds + (uint64_t)((mt * TGM_CHUNK + 2 * k16 * TGM_PLANE) >> 4);
-                        const uint32_t d = tmem_base + mt * 256;
-                        mma_f16(d, dAh, dB, IDESC2, (i | k16) != 0);                    // A_h0 * [B_h0 ; B_h1] -> [main | correction]
-                        mma_f16(d + 128, dAh + (uint64_t)(2048 >> 4), dB, IDESC1, 1);    // A_h1 * B_h0 -> correction
-                    }
-                }
-                if (CL == 1) mma_commit(&empty_bar[st]);
-                else mma_commit_mc(&empty_bar[st], CL_MASK);             // the stage of EVERY peer holds data this CTA multicast
-                if (i == nc - 1) mma_commit(&done_bar);
+            for (int k16 = 0; k16 < TGM_KC / 16; ++k16) {
+                const uint32_t sa = s0 + st * STAGE + w * 1024 + 2 * k16 * TGM_PLANE;
+                const uint64_t dA = smem_desc(sa, TGM_PLANE, 128);
+                const uint64_t dB = smem_desc(s0 + st * STAGE + TGM_CHUNK + 2 * k16 * TGM_PLANE, TGM_PLANE, 128);
+                wgmma_f16<128>(acc, dA, dB, 1);                                        // A_h0 * B_h0 -> main
+                wgmma_f16<128>(cor, dA, dB + (uint64_t)(2048 >> 4), 1);                // A_h0 * B_h1 -> correction
+                wgmma_f16<128>(cor, dA + (uint64_t)(2048 >> 4), dB, 1);                // A_h1 * B_h0 -> correction
             }
+            wgmma_commit();
+            wgmma_wait<1>();                                // the previous chunk's wgmmas have read their stage
             __syncwarp();
-        }
-    } else {
-        // ===== epilogue: part[split][m][n] = D[:, n] + 2^-11 * D[:, 128 + n] =====
-        const int ew = warp - 2, lq = warp & 3, half = ew >> 2;       // TMEM lane quarter = warp % 4 (hardware rule)
-        if (nc > 0) {
-            mbar_wait(&done_bar, 0);
-            fence_after_thread_sync();
-        }
-        float* P = part + (int64_t)split * M * N;
-#pragma unroll 1
-        for (int q = half; q < MT * 8; q += 2) {
-            const int mt = q >> 3, j = q & 7;
-            float v[16], v2[16];
-            if (nc > 0) {
-                __syncwarp();
-                const uint32_t t = tmem_base + ((uint32_t)(lq * 32) << 16) + (uint32_t)(mt * 256 + j * 16);
-                tmem_ld16_async(t, v);
-                tmem_ld16_async(t + 128, v2);
-                tmem_ld_wait();
-            } else {
-#pragma unroll
-                for (int x = 0; x < 16; ++x) v[x] = v2[x] = 0.0f;
+            if (i > 0 && lane == 0) {
+                const int ps = (i - 1) % TGM_STAGES;
+                if (CL == 1) mbar_arrive(&empty_bar[ps]);
+                else
+                    for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&empty_bar[ps], r);   // every peer's stage holds data this CTA multicast
             }
-            const int m = (mgroup * MT + mt) * 128 + lq * 32 + lane;
-            const int n = ntile * 128 + j * 16;
-            if (m < M) {
+        }
+        wgmma_wait<0>();
+        fence_regs<64>(acc);
+        fence_regs<64>(cor);
+        // ===== epilogue: part[split][m][n] = main + 2^-11 * correction =====
+        float* P = part + (int64_t)split * M * N;
 #pragma unroll
-                for (int x = 0; x < 16; x += 4) {
-                    if (n + x + 3 < N)
-                        *reinterpret_cast<float4*>(P + (int64_t)m * N + n + x) =
-                            make_float4(fmaf(v2[x], F16_LO_INV, v[x]), fmaf(v2[x + 1], F16_LO_INV, v[x + 1]),
-                                        fmaf(v2[x + 2], F16_LO_INV, v[x + 2]), fmaf(v2[x + 3], F16_LO_INV, v[x + 3]));
-                    else
-                        for (int y = 0; y < 4; ++y)
-                            if (n + x + y < N) P[(int64_t)m * N + n + x + y] = fmaf(v2[x + y], F16_LO_INV, v[x + y]);
-                }
+        for (int h = 0; h < 2; ++h) {
+            const int m = mtile * 128 + w * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            if (m >= M) continue;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int n = ntile * 128 + 8 * j + 2 * (lane & 3);        // N % 4 == 0: n < N implies n + 1 < N
+                if (n < N)
+                    *reinterpret_cast<float2*>(P + (int64_t)m * N + n) =
+                        make_float2(fmaf(cor[4 * j + 2 * h], F16_LO_INV, acc[4 * j + 2 * h]),
+                                    fmaf(cor[4 * j + 2 * h + 1], F16_LO_INV, acc[4 * j + 2 * h + 1]));
             }
         }
     }
-    fence_before_thread_sync();
-    __syncthreads();
     if (CL > 1) cluster_sync_all();                         // no CTA leaves while a peer may still arrive on its barriers
-    if (warp == 0) tmem_dealloc(tmem_base, TCOLS);
 }
 
 // W[K][N] (row-major, arbitrary element alignment) -> Wc[n tile][k octet][h0 | h1][128][8 x fp16]; columns >= N are zero
@@ -214,11 +187,11 @@ int dne_launch_theta_prep(const float* W, int K, int N, float* Wc, cudaStream_t 
     return 0;
 }
 
-template <int MT, int CL>
-static int launch_tgm(const float* Xc, const float* Wc, int M, int N, int KQ, int cps, int n_chunks, int n_split, int m_groups,
+template <int CL>
+static int launch_tgm(const float* Xc, const float* Wc, int M, int N, int KQ, int cps, int n_chunks, int n_split, int m_tiles,
                       int n_tiles, float* part, cudaStream_t st) {
-    constexpr int SMEM = TGM_STAGES * (MT + 1) * TGM_CHUNK + 256;
-    auto kern = theta_gemm_tma_kernel<MT, CL>;
+    constexpr int SMEM = TGM_STAGES * 2 * TGM_CHUNK + 256;
+    auto kern = theta_gemm_tma_kernel<CL>;
     int dev = 0;
     cudaGetDevice(&dev);
     static bool attr_done[64] = {};
@@ -227,7 +200,7 @@ static int launch_tgm(const float* Xc, const float* Wc, int M, int N, int KQ, in
         attr_done[dev] = true;
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(n_tiles, n_split, m_groups);          // blockIdx.x = N tile (= rank in the cluster when CL > 1)
+    cfg.gridDim = dim3(n_tiles, n_split, m_tiles);           // blockIdx.x = N tile (= rank in the cluster when CL > 1)
     cfg.blockDim = dim3(TGM_THREADS);
     cfg.dynamicSmemBytes = SMEM;
     cfg.stream = st;
@@ -250,13 +223,10 @@ int dne_launch_theta_gemm_tma(const float* Xc, const float* Wc, int M, int K, in
     if (!dne_tgm_supported(K, N, k_per_split)) return DNE_ERR_UNSUP;
     const int KQ = K / 8, n_chunks = K / TGM_KC, cps = k_per_split / TGM_KC;      // KQ: k-octet planes
     const int m_tiles = (M + 127) / 128, n_tiles = (N + 127) / 128;
-    if (m_tiles > 1 && (m_tiles & 1)) return DNE_ERR_UNSUP;          // M tiles come in pairs (one CTA owns two) or alone
-#define TGM_ARGS Xc, Wc, M, N, KQ, cps, n_chunks, n_split, (m_tiles >= 2 ? m_tiles / 2 : 1), n_tiles, part, st
-    // cluster multicast of the A chunk (g_dne_theta_mc, dne_set_option("theta_mc", 1)) measured SLOWER on B200 (32 us vs
-    // 18 us for the LargeModel fc at 256 slots: the 4-CTA cluster runs in lock step and must be co-scheduled): off
-    if (g_dne_theta_mc && m_tiles >= 2 && n_tiles == 4) return launch_tgm<2, 4>(TGM_ARGS);
-    if (g_dne_theta_mc && m_tiles >= 2 && n_tiles == 2) return launch_tgm<2, 2>(TGM_ARGS);
-    if (m_tiles >= 2) return launch_tgm<2, 1>(TGM_ARGS);
-    return launch_tgm<1, 1>(TGM_ARGS);
+#define TGM_ARGS Xc, Wc, M, N, KQ, cps, n_chunks, n_split, m_tiles, n_tiles, part, st
+    // cluster multicast of the A chunk (g_dne_theta_mc, dne_set_option("theta_mc", 1)): off by default (not measured faster)
+    if (g_dne_theta_mc && n_tiles == 4) return launch_tgm<4>(TGM_ARGS);
+    if (g_dne_theta_mc && n_tiles == 2) return launch_tgm<2>(TGM_ARGS);
+    return launch_tgm<1>(TGM_ARGS);
 #undef TGM_ARGS
 }

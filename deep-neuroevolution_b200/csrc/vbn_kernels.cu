@@ -9,7 +9,7 @@
 // because decay = 0), normalise, activate, continue.  This is the one sub-problem of the path with real weight
 // reuse per member (M = n_ref*441 rows per member for conv1): a dense contraction.
 //
-// r02: with conv_tc = 2 (default) the convolutions of the pass run on the shifted-window tcgen05 kernels of the tick
+// r02: with conv_tc = 2 (default) the convolutions of the pass run on the shifted-window wgmma kernels of the tick
 // (conv_s2d.cu) over n_slots * n_ref VIRTUAL slots (virtual slot v = image v % n_ref of member v / n_ref: consecutive CTAs
 // share a member, whose weight rows stay L2-hot), writing the raw pre-normalisation output as NHWC floats; after the batch
 // statistics, vbn_image_kernel normalises + activates and writes the NEXT conv layer's space-to-depth fp16-split image
@@ -17,7 +17,7 @@
 // the r01 tensor-core kernels, conv_tc = 0 the fp32 SIMT referee.
 #include "common.cuh"
 #include "forward.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
 __device__ __forceinline__ bool v_slot_active(const SlotArgs& a, int slot) { return !a.active || a.active[slot]; }
 __device__ __forceinline__ const float* v_slot_theta(const SlotArgs& a, int slot) {
@@ -284,7 +284,7 @@ vbn_image_kernel(SlotArgs sa, const float* __restrict__ Y, int64_t y_vslot_strid
             e[j] = apply_act(r, act);
         }
         uint4 hi, lo;
-        tc05::split_f16x8(e, hi, lo);
+        wg::split_f16x8(e, hi, lo);
         const int Yp = oy + g.nPADB, Xp = ox + g.nPADB;
         const int pix = (Yp / g.nS) * g.nW + (Xp / g.nS), pp = (Yp % g.nS) * g.nS + (Xp % g.nS);
         const int co = pp * no + q;
@@ -410,7 +410,7 @@ extern "C" int dne_vbn_reference_pass(dne_ctx* ctx, const dne_net_desc* net, con
             }
         } else {
             DNE_CHECK_ARG(!cur_u8 && L.cin == cur_elems && L.cin % 4 == 0, "dense layer input mismatch");
-            // tensor cores (tcgen05, 3xTF32: tc_conv.cu member_gemm_tc_kernel) unless conv_tc = 0 selects the fp32 SIMT referee
+            // tensor cores (wgmma, 3xTF32: tc_conv.cu member_gemm_tc_kernel) unless conv_tc = 0 selects the fp32 SIMT referee
             if (!(g_dne_conv_tc && dne_launch_member_gemm_tc(sa, L.off_w, pre_b, (const float*)cur, (int64_t)n_ref * cur_elems, n_ref,
                                                              L.cin, L.cout, out, out_slot_stride, n_slots, st) == 0)) {
                 dim3 grid((L.cout + MG_BN - 1) / MG_BN, (n_ref + MG_BM - 1) / MG_BM, n_slots);

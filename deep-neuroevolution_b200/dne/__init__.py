@@ -1,4 +1,4 @@
-"""dne -- host side of libdne.so: the sm_100a ES/GA rollout-and-update engine.
+"""dne -- host side of libdne.so: the sm_90a ES/GA rollout-and-update engine.
 
 Only what the hot path needs: the ctypes binding (`_ffi`), network descriptors (`nets`), the device noise slab
 (`noise`), the rollout/update engine (`engine`), the batched environment interface (`envs`) and population

@@ -107,14 +107,13 @@ def lib():
 
 _DEV_SIGS = {
     "dne_test_tc_gemm": [_P, _P, _P, C.c_int, C.c_int, _P],
-    "dne_probe_mma": [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P],
     "dne_dev_tc_window": [_P, _P, _P, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.c_int, _P],
 }
 _dev = None
 
 
 def dev_lib():
-    """libdne_dev.so: self-tests / micro-probes of the tcgen05 + TMA plumbing (csrc/dev/).  Tests and tools only; the
+    """libdne_dev.so: self-tests of the wgmma + TMA plumbing (csrc/dev/).  Tests and tools only; the
     product path never loads it."""
     global _dev
     if _dev is None:

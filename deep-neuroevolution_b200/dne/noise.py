@@ -4,7 +4,7 @@ Reference: es_distributed/es.py:51-67 (dup gpu_implementation/neuroevolution/hel
 ``noise = RandomState(123).randn(250_000_000)`` cast float64->float32 into fork-shared memory, ``get(i, dim)``
 returns the view ``noise[i:i+dim]``, ``sample_index(stream, dim) = stream.randint(0, len(noise)-dim+1)``.
 
-Here the table lives in HBM (1 GB of the 180 GB); every rank holds a full replica.  The values are generated
+Here the table lives in HBM (1 GB of the 80 GB); every rank holds a full replica.  The values are generated
 on the host with numpy's frozen legacy MT19937 / polar Box-Muller stream (bit-identical to the reference) and
 uploaded once.  Workers never ship weights or gradients, only (index, return) pairs -- the shared-seed trick of
 the reference is kept as is.

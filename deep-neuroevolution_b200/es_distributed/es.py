@@ -1,4 +1,4 @@
-"""``es_distributed.es`` -- the reference's ES driver API (es.py:12-23,26-85,125-138,141-353,366-439) on the B200 engine.
+"""``es_distributed.es`` -- the reference's ES driver API (es.py:12-23,26-85,125-138,141-353,366-439) on the H100 engine.
 
 Same names, argument meaning and configuration keys: ``Config``, ``Task``, ``Result``, ``RunningStat``,
 ``SharedNoiseTable``, ``compute_ranks``, ``compute_centered_ranks``, ``setup``, ``run_master``, ``run_worker``.

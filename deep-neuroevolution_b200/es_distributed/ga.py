@@ -1,4 +1,4 @@
-"""``es_distributed.ga`` -- the reference's GA driver (ga.py:4,33-206,209-284) on the B200 engine, plus the GPU path's
+"""``es_distributed.ga`` -- the reference's GA driver (ga.py:4,33-206,209-284) on the H100 engine, plus the GPU path's
 Deep GA options (gpu_implementation/ga.py:123-129,165-204,260-271; configurations/ga_atari_config.json).
 
 Genomes are seed chains (ga.py:252-254): ``[idx0, idx1, ...]``; weights = reinitialize(noise[idx0]) + sigma * sum

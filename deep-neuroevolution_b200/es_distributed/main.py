@@ -1,4 +1,4 @@
-"""``python -m es_distributed.main`` -- the reference CLI (es_distributed/main.py:29-86) on the B200 engine.
+"""``python -m es_distributed.main`` -- the reference CLI (es_distributed/main.py:29-86) on the H100 engine.
 
   master   --algo {es,ns-es,nsr-es,ga,rs}  --exp_file / --exp_str  [--master_socket_path] [--log_dir]
   workers  --algo ... --master_host --master_port --relay_socket_path --num_workers
@@ -87,7 +87,7 @@ def master(algo, exp_str, exp_file, master_socket_path, log_dir, max_iterations,
 @click.option('--num_workers', type=int, default=0)
 def workers(algo, master_host, master_port, relay_socket_path, num_workers):
     # main.py:64-86: forks a redis relay and num_workers rollout processes sharing one noise table.
-    logging.info("es_distributed (B200 engine): rollout workers are the GPU ranks of the `master` torchrun job "
+    logging.info("es_distributed (H100 engine): rollout workers are the GPU ranks of the `master` torchrun job "
                  "(population sharded over NCCL); there is no redis relay to attach to -- nothing to do.")
 
 

@@ -1,4 +1,4 @@
-"""``es_distributed.nses`` -- NS-ES / NSR-ES (nses.py:12-39,58-316,318-400) on the B200 engine.
+"""``es_distributed.nses`` -- NS-ES / NSR-ES (nses.py:12-39,58-316,318-400) on the H100 engine.
 
 Kept semantics: a meta-population of ``novelty_search.population_size`` (theta, optimizer) pairs (nses.py:95-117), an
 archive of behaviour characterisations seeded with each member's mean BC (:113-114); every iteration runs one ES

@@ -1,4 +1,4 @@
-"""``es_distributed.rs`` -- the reference's random-search driver (rs.py:4-174) on the B200 engine.
+"""``es_distributed.rs`` -- the reference's random-search driver (rs.py:4-174) on the H100 engine.
 
 Random search evaluates ``episodes_per_batch`` fresh candidates per iteration, each candidate being
 ``reinitialize(noise[idx])`` (rs.py:112-116 on the master, ga.py:256-260 in the workers it reuses: a GA genome of

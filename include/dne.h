@@ -1,4 +1,4 @@
-/* dne.h -- C ABI of libdne.so: the sm_100a ES/GA rollout-and-update engine.
+/* dne.h -- C ABI of libdne.so: the sm_90a ES/GA rollout-and-update engine.
  *
  * The reference (uber-research/deep-neuroevolution) is Python and has no C ABI for this path; its
  * "plugin boundary" is (a) the Python API es_distributed.{es,ga,nses}.run_master/run_worker +
@@ -94,8 +94,8 @@ int         dne_abi_sizes(int* layer_desc_bytes, int* net_desc_bytes);
  * (dense_noise_gemv) on the stream it is launched on; read() synchronises the device. */
 long long   dne_launch_count(int reset);
 /* Runtime switches (process-wide; A/B measurement and referee paths only):
- *   "conv_tc" = 2 (default): shifted-window tcgen05 convolutions, images / weights by TMA (conv_s2d.cu), also used by the
- *               virtual-batch-norm reference pass; 1: im2col-staged tcgen05 kind::tf32 convolutions (tc_conv.cu); 0: fp32 SIMT
+ *   "conv_tc" = 2 (default): shifted-window wgmma convolutions, images / weights by TMA (conv_s2d.cu), also used by the
+ *               virtual-batch-norm reference pass; 1: im2col-staged wgmma tf32 convolutions (tc_conv.cu); 0: fp32 SIMT
  *               kernels everywhere (the parity referee).
  *   "theta_tma" = 1 (default): TMA-fed shared-theta GEMM when a prepared region is current (dne_theta_prepare).
  *   "theta_mc" = 0 (default): cluster-multicast variant of it (measured slower).

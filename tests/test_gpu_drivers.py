@@ -402,3 +402,34 @@ def test_mujoco_discretised_action_heads():
     assert pc.net.n_out == 3 * 4
     a = pc.action_fn(np.eye(4, dtype=np.float32)[[1, 3, 0]].reshape(1, 12))
     np.testing.assert_allclose(a[0], [-0.2, 1.0, 0.0], rtol=1e-6)
+
+
+def test_bench_without_warmup_prints_line_and_dumps_seeded_outputs(tmp_path):
+    """bench.py at a tiny size with --warmup 0 (the e2e window opens before run_master's first iteration) prints its one
+    JSON line; the timed region's kernel launches scale with --steps (two timed generations launch exactly twice what one
+    does); --dump-outputs writes the last generation's arrays (float32, <= 64 MB, actions = argmax of the dumped logits);
+    a second run with the same arguments sees the same inputs and computes the same outputs."""
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+    def bench(steps, d):
+        out = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--gpus", "1", "--steps", str(steps), "--warmup", "0",
+                              "--pop", "8", "--episode-len", "20", "--noise-count", str(NOISE_COUNT), "--no-cpu-baseline",
+                              "--dump-outputs", str(d)], capture_output=True, text=True, timeout=600)
+        assert out.returncode == 0, out.stderr[-3000:]
+        line = json.loads(out.stdout.strip().splitlines()[-1])
+        assert line["steps"] == steps and line["warmup"] == 0 and line["value"] > 0 and line["e2e"]["value"] > 0
+        return line, {k: np.load(d / f"{k}.npy") for k in ("theta", "grad", "returns", "logits", "actions")}
+
+    one, _ = bench(1, tmp_path / "d1")
+    two, a = bench(2, tmp_path / "d2")
+    again, b = bench(2, tmp_path / "d3")
+    assert one["gpu_launches"] > 0 and two["gpu_launches"] == 2 * one["gpu_launches"]
+    assert a["theta"].shape == (4052658,) and a["grad"].shape == (4052658,) and a["returns"].shape == (4, 2)
+    assert a["logits"].shape == (8, 18) and a["actions"].shape == (8,)
+    assert all(v.dtype == np.float32 for v in a.values()) and sum(v.nbytes for v in a.values()) <= 64 << 20
+    np.testing.assert_array_equal(a["actions"], np.argmax(a["logits"], axis=1))
+    assert np.abs(a["grad"]).max() > 0
+    for k in a:
+        np.testing.assert_array_equal(a[k], b[k], err_msg=k)

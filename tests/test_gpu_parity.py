@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI of libdne.so) against the CPU oracle and the committed
-golden vectors generated from the reference's own numpy code.  Run on the B200 box: pytest -m gpu.
+golden vectors generated from the reference's own numpy code.  Run on an H100: pytest -m gpu.
 
 Tolerances (stated once):
   * integer / index / rank / selection bookkeeping: bit-exact

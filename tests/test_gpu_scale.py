@@ -3,7 +3,7 @@ antithetic pairs + an inactive tail (the last wave of pop 1000), the 124-slot sh
 phase-event schedule, and the ESAtariPolicy virtual-batch-norm pass at the configuration's n_ref = 128.
 
 What these cover that the small-slot tests cannot (VERDICT r01 weak-1): every persistent CTA of the noise GEMV walks
-several (pair, K-chunk) work items (n_items = 128 groups x 32 chunks = 4096 >> the 296-CTA grid) with inactive items
+several (pair, K-chunk) work items (n_items = 128 groups x 32 chunks = 4096 >> the 264-CTA grid) with inactive items
 skipped inside the loop; the conv / theta-GEMM grids run more than one wave; split-K of the shared-theta GEMM at
 M = 256.  Oracle on a sample of slots (the oracle is a CPU torch forward: ~20 ms per slot), SIMT-vs-tensor-core cross
 check on ALL slots.  Tolerance: |dlogit|_inf <= 2e-5 * max(1, |logit|_inf) per row (tests/test_gpu_parity.py)."""
@@ -26,7 +26,7 @@ from dne.noise import SharedNoiseTable    # noqa: E402
 DEV = torch.device("cuda", 0)
 NOISE_COUNT = 12_000_000
 SIGMA = 0.005                             # configurations/frostbite_es.json:7
-GEMV_GRID = 2 * 148                       # persistent CTAs of gemv_bulk_kernel (2 per SM)
+GEMV_GRID = 2 * 132                       # persistent CTAs of gemv_bulk_kernel (2 per SM of an H100 SXM)
 
 
 @pytest.fixture(scope="module")

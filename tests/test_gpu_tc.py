@@ -1,5 +1,5 @@
-"""GPU tests of the tensor-core (tcgen05 / TMEM, 3xTF32) convolution path against the oracle and against the
-fp32 SIMT path, plus GA slots (per-slot parent rows) and a self-test of the tcgen05 plumbing."""
+"""GPU tests of the tensor-core (wgmma, 3xTF32 / 2 x fp16) convolution path against the oracle and against the
+fp32 SIMT path, plus GA slots (per-slot parent rows) and a self-test of the wgmma plumbing."""
 import ctypes as C
 
 import numpy as np
@@ -36,8 +36,8 @@ def cuda(x):
 
 @pytest.mark.parametrize("n,k", [(32, 256), (64, 512), (64, 576), (16, 256), (32, 32)])
 def test_tcgen05_gemm_selftest(n, k):
-    """C = A B^T through the hand-written tcgen05 path (smem descriptors, instruction descriptor, TMEM alloc/ld,
-    mbarrier commit) with the 3xTF32 split: must be fp32-accurate, not TF32-accurate."""
+    """C = A B^T through the hand-written wgmma path (smem descriptors, register accumulators, wgmma fence / commit /
+    wait) with the 3xTF32 split: must be fp32-accurate, not TF32-accurate."""
     rs = np.random.RandomState(n * 1000 + k)
     A = rs.randn(128, k).astype(np.float32)
     B = rs.randn(n, k).astype(np.float32)
@@ -75,8 +75,8 @@ def test_conv_tc_vs_simt_vs_oracle(ctx, host_noise, name):
     pidx = rs.randint(0, NOISE_COUNT - P + 1, size=n_slots // 2).astype(np.int64)
     idx, scale = np.repeat(pidx, 2), np.tile([0.02, -0.02], n_slots // 2).astype(np.float32)
     obs = rs.randint(0, 256, size=(n_slots, 84, 84, 4)).astype(np.uint8)
-    l2, a2 = _forward(ctx, net, theta, idx, scale, obs, 1, 2)        # shifted-window tcgen05 + TMA (default)
-    lt, at = _forward(ctx, net, theta, idx, scale, obs, 1, 1)        # im2col-staged tcgen05
+    l2, a2 = _forward(ctx, net, theta, idx, scale, obs, 1, 2)        # shifted-window wgmma + TMA (default)
+    lt, at = _forward(ctx, net, theta, idx, scale, obs, 1, 1)        # im2col-staged wgmma
     ls, as_ = _forward(ctx, net, theta, idx, scale, obs, 1, 0)       # fp32 SIMT
     ref = np.stack([O.forward(net_o, O.perturb(theta, host_noise, int(idx[s]), 0.02, 1 if scale[s] > 0 else -1),
                               obs[s:s + 1])[0][0] for s in range(n_slots)])
@@ -302,7 +302,7 @@ def test_theta_gemm_tma_vs_thread_staged_and_invalidation(ctx, host_noise):
 
 @pytest.mark.parametrize("name", ["ESAtariPolicy", "ModelVirtualBN"])
 def test_vbn_reference_pass_tensor_core_paths_match_simt(ctx, host_noise, name):
-    """The virtual-batch-norm reference pass (policies.py:322-328,399) three ways: conv_tc = 2 (shifted-window tcgen05
+    """The virtual-batch-norm reference pass (policies.py:322-328,399) three ways: conv_tc = 2 (shifted-window wgmma
     convolutions over n_slots * n_ref virtual slots + fp16-split images + tensor-core member GEMM), conv_tc = 1 (r01
     tensor-core kernels) and conv_tc = 0 (fp32 SIMT referee): same statistics, and the tick on those statistics gives the
     same logits.  Ragged sizes: n_ref not a multiple of anything, an inactive slot in the middle, unpaired scales."""

@@ -1,5 +1,5 @@
 """Dev tool (GPU box): time of the virtual-batch-norm reference pass (256 members x 128 reference observations) per
-conv_tc mode (2 = shifted-window tcgen05 convs over virtual slots + tensor-core member GEMM, 1 = r01 tensor-core kernels,
+conv_tc mode (2 = shifted-window wgmma convs over virtual slots + tensor-core member GEMM, 1 = r01 tensor-core kernels,
 0 = fp32 SIMT).  Not a bench."""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -203,7 +203,7 @@ def run(args, emit, ClockSampler, load_peaks):
     launches_per_tick = max(len(dense), 1)
     avg_ms = tot.value / max(n_t.value, 1)
     achieved = (bytes_per_tick / launches_per_tick) / (avg_ms * 1e-3) / 1e9 if n_t.value else None
-    roofline = {"bound": "hbm", "kernel": "gemv_bulk_kernel (noise GEMV of the decomposed dense layers)",
+    roofline = {"bound": "hbm", "kernel": "gemv_union_kernel (noise GEMV of the decomposed dense layers)",
                 "achieved": achieved, "peak": peaks["hbm_gbs"], "peak_source": peak_src, "unit": "GB/s",
                 "frac": achieved / peaks["hbm_gbs"] if achieved else None, "traffic": None,
                 "launches_timed": n_t.value, "avg_launch_ms": avg_ms,

@@ -79,15 +79,12 @@ extern "C" int dne_set_option(const char* name, int value) {
     if (strcmp(name, "conv_tc") == 0 && value >= 0 && value <= 2) { g_dne_conv_tc = value; return DNE_OK; }
     if (strcmp(name, "gemv_bulk") == 0) { g_dne_gemv_bulk = value ? 1 : 0; return DNE_OK; }
     if (strcmp(name, "fuse_head") == 0) { g_dne_fuse_head = value ? 1 : 0; return DNE_OK; }
-    if (strcmp(name, "gemv_chunk_kb") == 0 && value >= 64 && value <= 4096) { extern int g_dne_gemv_chunk_kb; g_dne_gemv_chunk_kb = value; return DNE_OK; }
     if (strcmp(name, "theta_mc") == 0) { extern int g_dne_theta_mc; g_dne_theta_mc = value ? 1 : 0; return DNE_OK; }
     if (strcmp(name, "theta_tma") == 0) { g_dne_theta_tma = value ? 1 : 0; return DNE_OK; }
     if (strcmp(name, "gemv_stages") == 0 && value >= 2 && value <= 8) { extern int g_dne_gemv_stages; g_dne_gemv_stages = value; return DNE_OK; }
-    if (strcmp(name, "gemv_prefetch") == 0 && value >= 0 && value <= 256) { extern int g_dne_gemv_prefetch; g_dne_gemv_prefetch = value; return DNE_OK; }
     if (strcmp(name, "fold_theta") == 0 && value >= 0 && value <= 1) { g_dne_fold_theta = value; return DNE_OK; }
     if (strcmp(name, "chain_ticks") == 0 && value >= 0 && value <= 1) { g_dne_chain_ticks = value; return DNE_OK; }
     if (strcmp(name, "pdl") == 0 && value >= 0 && value <= 1) { g_dne_pdl = value; return DNE_OK; }
-    if (strcmp(name, "gemv_balance") == 0 && value >= 0 && value <= 1) { extern int g_dne_gemv_balance; g_dne_gemv_balance = value; return DNE_OK; }
     if (strcmp(name, "gemv_grid") == 0 && value >= 0) { extern int g_dne_gemv_grid; g_dne_gemv_grid = value; return DNE_OK; }
     if (strcmp(name, "gemv_ctas_per_sm") == 0 && value >= 1 && value <= 2) { g_dne_gemv_ctas_per_sm = value; return DNE_OK; }
     dne_set_error("dne_set_option: unknown option '%s'", name);

@@ -30,17 +30,21 @@ struct GemvSrc {
 extern int g_dne_gemv_bulk;
 extern int g_dne_fold_theta;
 extern int g_dne_gemv_ctas_per_sm;
-// TMA-bulk-copy pipelined variant of the noise GEMV (gemv_bulk.cu).  Returns DNE_ERR_UNSUP if the shape is not covered.
 int dne_launch_member_gemm_tc(const SlotArgs& sa, int64_t off_w, int64_t off_b, const float* X, int64_t x_slot_stride, int M,
                               int K, int N, float* out, int64_t out_slot_stride, int n_slots, cudaStream_t st);
-int dne_launch_gemv_bulk(const SlotArgs& sa, const GemvSrc& src, int G, const float* X, int64_t x_slot_stride, int K,
-                         int N, int rows_per_chunk, int n_chunks, int n_slots, float* part, int sm_count,
-                         cudaStream_t st, const float* fold_theta = nullptr, int fold_n_split = 0);
-bool dne_gemv_bulk_can_fold(int G, int N, int n_chunks, int n_split);
+// Union GEMV (gemv_bulk.cu): the table is cut into blocks of DNE_GEMV_BLOCK_ROWS rows of N floats, each covered block is
+// streamed once per launch through a cp.async.bulk ring and applied to every group whose slice intersects it.  Each group
+// writes dne_gemv_pieces(K) partials [group][piece][G][N].  Returns DNE_ERR_UNSUP if the shape is not covered.
+constexpr int DNE_GEMV_BLOCK_ROWS = 256;
+int dne_gemv_pieces(int K);
+int dne_launch_gemv_union(const SlotArgs& sa, const GemvSrc& src, int G, const float* X, int64_t x_slot_stride, int K,
+                          int N, int n_pieces, int n_slots, float* part, int sm_count, cudaStream_t st,
+                          const float* fold_theta = nullptr, int fold_n_split = 0);
 
 struct DensePlan {
     bool decomposed;
     int n_split, k_per_split;     // theta GEMM split-K
+    // n_chunks: partials per group (dne_gemv_pieces); rows_per_chunk: K rows per partial of the SIMT GEMV
     int G, Gt, rows_per_chunk, n_chunks, rw;     // Gt: theta group size (0 = shared theta GEMM)
     size_t part_theta_floats, part_noise_floats;
 };

@@ -656,23 +656,6 @@ int dne_launch_conv_layer_simt(const SlotArgs& sa, const dne_layer_desc& L, cons
 }
 
 // ---- dense-layer planning (shared by the ws query and the launcher) -----------------------------------
-int g_dne_gemv_chunk_kb = 1024;    // dne_set_option("gemv_chunk_kb", v): bytes of weights per GEMV work item (and per partial)
-static int pick_rows_per_chunk(int K, int N, int groups, int sm_count) {
-    // target ~1 MB of noise per work item (persistent bulk-copy GEMV; r02 A/B: same GEMV time as 512 KB, half the partials
-    // for the combine kernel to read), prefer exact divisors of K
-    // ... but keep >= ~6 work items per persistent CTA (2 per SM): with fewer, the last partial round of the static
-    // schedule costs more than the halved partial traffic saves (62 pairs x 16 items = 3.35 per CTA -> 84 % busy)
-    size_t chunk_bytes = (size_t)g_dne_gemv_chunk_kb * 1024;
-    while (chunk_bytes > 256 * 1024 && (size_t)groups * ((size_t)K * N * 4 / chunk_bytes) < (size_t)12 * sm_count) chunk_bytes /= 2;
-    int target = (int)(chunk_bytes / ((size_t)N * 4));
-    if (target > 512) target = 512;           // GB_MAX_ROWS of gemv_bulk.cu (x staging buffer)
-    if (target < 8) target = 8;
-    if (target >= K) return K;
-    for (int r = target; r >= target / 2 && r >= 1; --r)
-        if (K % r == 0) return r;
-    return target;
-}
-
 DensePlan dne_plan_dense(const dne_layer_desc& L, int n_slots, int paired, bool shared_theta, int sm_count) {
     DensePlan p;
     memset(&p, 0, sizeof(p));
@@ -695,8 +678,10 @@ DensePlan dne_plan_dense(const dne_layer_desc& L, int n_slots, int paired, bool 
     kt_per += kt_per & 1;                                // k_per_split % 32 == 0: the TMA-fed fp16 GEMM moves K chunks of 32
     p.k_per_split = kt_per * DG_BK;
     p.n_split = (K + p.k_per_split - 1) / p.k_per_split;
-    p.rows_per_chunk = pick_rows_per_chunk(K, N, (n_slots + p.G - 1) / p.G, sm_count);
-    p.n_chunks = (K + p.rows_per_chunk - 1) / p.rows_per_chunk;
+    // partials per group: the union GEMV's pieces (one per table block a slice can touch); the SIMT GEMV writes the same
+    // number of partials, each over rows_per_chunk rows of K
+    p.n_chunks = dne_gemv_pieces(K);
+    p.rows_per_chunk = (K + p.n_chunks - 1) / p.n_chunks;
     const int nq = N / 4;
     p.rw = 1;
     while (nq * p.rw * 2 <= 256 && p.rw * 2 <= 8) p.rw *= 2;
@@ -747,8 +732,8 @@ int dne_launch_dense_layer(const dne_ctx* ctx, const SlotArgs& sa, const dne_lay
     } else {
         GemvSrc ts{sa.theta, nullptr, sa.theta_idx, sa.P, L.off_w};
         dim3 grid(p.n_chunks, (n_slots + p.Gt - 1) / p.Gt);
-        if (g_dne_gemv_bulk && dne_launch_gemv_bulk(sa, ts, p.Gt, X, x_slot_stride, K, N, p.rows_per_chunk, p.n_chunks,
-                                                    n_slots, part_theta, ctx->sm_count, st) == 0) {
+        if (g_dne_gemv_bulk && dne_launch_gemv_union(sa, ts, p.Gt, X, x_slot_stride, K, N, p.n_chunks, n_slots, part_theta,
+                                                     ctx->sm_count, st) == 0) {
         } else if (p.Gt == 2)
             dense_noise_gemv_kernel<2, 8><<<grid, threads, gemv_smem(2), st>>>(sa, ts, X, x_slot_stride, K, N,
                                                                               p.rows_per_chunk, part_theta);
@@ -773,12 +758,11 @@ int dne_launch_dense_layer(const dne_ctx* ctx, const SlotArgs& sa, const dne_lay
         dim3 grid(p.n_chunks, groups);
         const bool prof = ctx->prof_on && ctx->ev_n < ctx->ev_cap;
         if (prof) cudaEventRecord(ctx->ev[2 * ctx->ev_n], st);
-        // fold the theta GEMM's split-K partials into the GEMV output (gemv_bulk.cu) when the shapes allow it
-        folded = g_dne_gemv_bulk && g_dne_fold_theta && p.Gt == 0 && dne_gemv_bulk_can_fold(p.G, N, p.n_chunks, p.n_split) &&
-                 p.rows_per_chunk * N >= 192 * 1024;   // >= 768 KB items: with the 512 KB items of small tables the fold costs 0.8 us (A/B, tools/ab_tick.py)
-        if (g_dne_gemv_bulk && dne_launch_gemv_bulk(sa, ns, p.G, X, x_slot_stride, K, N, p.rows_per_chunk, p.n_chunks,
-                                                    n_slots, part_noise, ctx->sm_count, st, folded ? part_theta : nullptr,
-                                                    folded ? p.n_split : 0) == 0) {
+        // fold the theta GEMM's split-K partials into the GEMV output (gemv_bulk.cu)
+        folded = g_dne_gemv_bulk && g_dne_fold_theta && p.Gt == 0;
+        if (g_dne_gemv_bulk && dne_launch_gemv_union(sa, ns, p.G, X, x_slot_stride, K, N, p.n_chunks, n_slots, part_noise,
+                                                     ctx->sm_count, st, folded ? part_theta : nullptr,
+                                                     folded ? p.n_split : 0) == 0) {
         } else if ((folded = false), p.G == 2)
             dense_noise_gemv_kernel<2, 8><<<grid, threads, gemv_smem(2), st>>>(sa, ns, X, x_slot_stride, K, N,
                                                                               p.rows_per_chunk, part_noise);

@@ -1,17 +1,29 @@
-// gemv_bulk.cu -- the HBM-bound noise GEMV with a TMA bulk-copy (cp.async.bulk) shared-memory pipeline.
+// gemv_bulk.cu -- the HBM-bound GEMV of the decomposed dense layers, streaming the UNION of a launch's weight slices once.
 //
-// Same math and partial layout as dense_noise_gemv_kernel (forward_kernels.cu):
-//     part[group][chunk][g][n] = sum_{k in chunk} x_g[k] * W[k][n],   W = slab[E0 + k*N + n], E0 arbitrary alignment
-// but the weight rows do not pass through registers on their way in: a producer warp streams the 16B-ALIGNED superset
-// of the chunk (contiguous RB-row blocks, one cp.async.bulk each) into a ring of shared-memory stages, completion
-// tracked by mbarriers (full / empty), and 8 consumer warps read the rows back with conflict-free LDS.128.  The bytes
-// in flight are STAGES x 16 KB per CTA regardless of register allocation (the plain-LDG kernel is limited by how many
-// loads ptxas keeps in flight: measured 64 % of HBM peak; Little's law wants > 44 KB per SM).
-// CTAs are persistent: a static round-robin over (group, chunk) work items, the ring runs across item boundaries.
+// Same math as dense_noise_gemv_kernel (forward_kernels.cu): for every group of G slots that share one slice,
+//     y_g[n] = sum_k x_g[k] * W[k][n],   W = base[E0 + k*N + n],   E0 = idx[slot0] + off (arbitrary alignment)
+// The slices of one launch start at unrelated offsets of one table (noise slab, or the theta matrix for GA parents) and
+// overlap: 128 random 15.9 MB fc slices of the 1 GB noise table cover it about 2 times over.  Streaming every slice on
+// its own reads each covered byte ~2.3 times, and L2 (50 MB) absorbs almost none of it.  This kernel cuts the table into
+// a fixed grid of rows of N floats (aligned to the table base), groups the rows into blocks of GU_BLK rows, and makes every
+// block that some active group's slice intersects one work item: the item streams the block's covered rows ONCE into a
+// shared-memory ring (producer warp, cp.async.bulk, full / empty mbarriers) and applies them to every covering group.
 //
-// Alignment trick (see forward_kernels.cu): thread t always owns aligned column quad q = 4t..4t+3.  Element (r, q) of
-// the aligned stream is weight (k = r, n = q - a) for q >= a and (k = r - 1, n = N + q - a) for q < a, a = E0 & 3.
-// Only quad 0 has the second kind; it keeps a second accumulator fed from the SAME staged rows with multiplier x[r-1].
+// Row R, table column c of group g (R_g = E0_g div N, rho_g = E0_g mod N) is weight
+//     k = R - R_g - [c < rho_g],   n = (c - rho_g) mod N.
+// Consumer thread t owns column quad 4t..4t+3 of every row, so for each group its four components always feed the same four
+// outputs (rotated by rho_g), with multiplier x[k] or x[k-1].  x is staged per item over the block's rows, zero outside
+// [0, K) -- rows of the block that a group does not cover contribute exactly zero.  Each staged float4 is read from shared
+// memory once and used for every covering group (at most GU_VEC / G groups per pass; a block with more covering groups is
+// streamed again for the rest).
+//
+// Partials: group g's piece i is block floor(R_g / GU_BLK) + i, written to part[group][i][G][N] for i < M (dne_gemv_pieces);
+// pieces the group does not reach are written as zero.  The combine kernels add the M pieces in order: deterministic.
+//
+// The plan (which blocks, which groups cover each) depends only on the slot table, which nothing inside a tick writes, so
+// every CTA derives it in its prologue -- before griddepcontrol.wait -- from the <= n_groups intervals: no host sync, and it
+// cannot go stale when a caller rewrites the index tensors.  Items are dealt round-robin over the persistent CTAs.
+#include <climits>
 #include "common.cuh"
 #include "forward.cuh"
 #include "epilogue.cuh"
@@ -21,41 +33,70 @@ using namespace wg;
 
 int g_dne_gemv_bulk = 1;
 int g_dne_gemv_ctas_per_sm = 2;
-int g_dne_gemv_balance = 1;          // choose the grid size that balances the round-robin item deal (dne_set_option("gemv_balance"))
 int g_dne_gemv_grid = 0;             // > 0: cap on the number of CTAs (dne_set_option("gemv_grid")): leaves whole SMs to another stream
-int g_dne_gemv_stages = 6;           // shared-memory ring depth (2..GB_STAGES), dne_set_option("gemv_stages")
-int g_dne_gemv_prefetch = 0;         // L2 prefetch distance in stages (cp.async.bulk.prefetch.L2), dne_set_option("gemv_prefetch")
+int g_dne_gemv_stages = 5;           // shared-memory ring depth upper bound (2..GB_STAGES), dne_set_option("gemv_stages")
 
 constexpr int GB_CONSUMERS = 256;
 constexpr int GB_THREADS = GB_CONSUMERS + 32;      // + one producer warp
 constexpr int GB_STAGES = 8;                       // maximum ring depth (barrier arrays); the launch picks n_stages <= this
 constexpr int GB_STAGE_BYTES = 16384;
 constexpr int GB_RPR = 4;                          // rows per reader per stage: (16384/4N) / (256/(N/4)) = 4 for every N
-constexpr int GB_FOLD_O = 4, GB_FOLD_S = 3;         // fold: outputs per consumer thread (G*N <= 1024), theta splits per chunk
-constexpr int GB_MAX_ROWS = 512;                   // rows per work item (x staging buffer)
+constexpr int GU_BLK = DNE_GEMV_BLOCK_ROWS;        // table rows per block (work item)
+constexpr int GU_VEC = 8;                          // x vectors (covering groups x G) per pass: accumulator registers / 4
+constexpr int GU_VB = 4;                           // x vectors per round of the cross-reader reduction
+constexpr int GU_MIN_N = 64;                       // rows per stage 4096 / N <= 64
+constexpr int GU_XS_LD_MAX = GU_BLK + 4096 / GU_MIN_N;
+// shared array of the x staging [GU_VEC][XS_LD] and, after a pass's last stage, of the reduction [RW][GU_VB][N + 4]
+constexpr int GU_XS_FLOATS = GU_VEC * GU_XS_LD_MAX > (1024 / GU_MIN_N) * GU_VB * (GU_MIN_N + 4)
+                                 ? GU_VEC * GU_XS_LD_MAX : (1024 / GU_MIN_N) * GU_VB * (GU_MIN_N + 4);
+constexpr int GU_PLAN_BYTES_PER_GROUP = 8 + 5 * 4; // E0, b0, b1, sorted, start, prefix
+
+// Lists (one warp) the groups covering block b whose ordinal among them lies in [first, first + cap) into out[], in group
+// order; returns the total number of covering groups.
+__device__ __forceinline__ int gu_cover(const int* pb0, const int* pb1, int n_groups, int b, int first, int cap, int* out,
+                                        int lane) {
+    int total = 0;
+    for (int h0 = 0; h0 < n_groups; h0 += 32) {
+        const int h = h0 + lane;
+        const bool c = h < n_groups && pb0[h] <= b && b <= pb1[h];
+        const unsigned m = __ballot_sync(0xffffffffu, c);
+        const int ord = total + __popc(m & ((1u << lane) - 1u));
+        if (c && ord >= first && ord < first + cap) out[ord - first] = h;
+        total += __popc(m);
+    }
+    __syncwarp();
+    return total;
+}
 
 template <int G>
-__global__ void __launch_bounds__(GB_THREADS)
-gemv_bulk_kernel(SlotArgs sa, GemvSrc src, const float* __restrict__ X, int64_t x_slot_stride, int K, int N,
-                 int rows_per_chunk, int n_chunks, int n_groups, float* __restrict__ part, int n_stages, int pf_dist,
-                 const float* __restrict__ tpart, int t_split, int n_slots) {
+__global__ void __launch_bounds__(GB_THREADS, 2)
+gemv_union_kernel(SlotArgs sa, GemvSrc src, const float* __restrict__ X, int64_t x_slot_stride, int K, int N,
+                  int n_pieces, int n_groups, int n_slots, float* __restrict__ part, int n_stages,
+                  const float* __restrict__ tpart, int t_split) {
     // tpart != nullptr ("fold"): the shared-theta GEMM's split-K partials [t_split][n_slots][N] are folded into this
-    // kernel's output, part[group][chunk][g][n] = s_g * (noise partial of the chunk) + sum_{j = chunk (mod n_chunks)} tpart[j]:
-    // the combine kernel then adds n_chunks values per output instead of n_chunks + t_split (its latency-bound L2 round
-    // trips were 5 of 7 for the theta partials).  The <= GB_FOLD_S loads per output are issued at the top of the item and
-    // consumed after its last stage.  Fixed summation order: deterministic.
+    // kernel's output, part[group][piece][g][n] = s_g * (noise partial of the piece) + sum_{j = piece (mod n_pieces)} tpart[j]:
+    // the combine kernel then adds n_pieces values per output instead of n_pieces + t_split.  Fixed summation order.
+    constexpr int CAP = GU_VEC / G;                    // covering groups per pass
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
     float* stage_base = reinterpret_cast<float*>(smem);
-    float* red = reinterpret_cast<float*>(smem + n_stages * GB_STAGE_BYTES);        // [RW][G][N+4]
+    int64_t* pE0 = reinterpret_cast<int64_t*>(smem + n_stages * GB_STAGE_BYTES);
+    int* pb0 = reinterpret_cast<int*>(pE0 + n_groups);      // first / last block of each group (INT_MAX / -1: inactive)
+    int* pb1 = pb0 + n_groups;
+    int* psort = pb1 + n_groups;                             // groups by (first block, index)
+    int* pstart = psort + n_groups;                          // first block sorted entry i adds to the union
+    int* ppre = pstart + n_groups;                           // blocks added by the sorted entries before i
     __shared__ uint64_t full_bar[GB_STAGES], empty_bar[GB_STAGES];
-    __shared__ float xs[G][GB_MAX_ROWS + 8];           // xs[g][1 + r] = x_g[k_beg + r];  xs[g][0] = x_g[k_beg - 1]
+    __shared__ __align__(16) float xs[GU_XS_FLOATS];   // xs[v][1 + L] = x_v[k] at block row L; reused by the reduction
+    __shared__ int cov_c[CAP], cov_p[CAP];                  // this pass's groups: consumers / producer
+    __shared__ int rho_c[CAP];
+    __shared__ int s_total, s_row0, s_nelem, s_items;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NQ = N >> 2;
     const int RW = GB_CONSUMERS / NQ;                  // row readers per stage
     const int RB = GB_RPR * RW;                        // rows per stage
-    const int n_items = n_groups * n_chunks;
+    const int XS_LD = GU_BLK + RB;
     pdl_trigger();                                     // common.cuh: PDL chain of the tick
 
     if (tid == 0) {
@@ -65,60 +106,106 @@ gemv_bulk_kernel(SlotArgs sa, GemvSrc src, const float* __restrict__ X, int64_t 
         }
         fence_mbar_init();
     }
-    __syncthreads();
-
-    auto item_active = [&](int item) {
-        const int slot0 = (item / n_chunks) * G;
+    // ---- plan, step 1: every group's slice start and block interval ----
+    for (int g = tid; g < n_groups; g += GB_THREADS) {
+        const int slot0 = g * G;
         bool any = false;
 #pragma unroll
-        for (int g = 0; g < G; ++g) any = any || slot_active(sa, slot0 + g);
-        return any;
-    };
-    auto item_base = [&](int item, int& k_beg, int& rows, int& a) -> const float* {
-        const int group = item / n_chunks, chunk = item % n_chunks;
-        const int slot0 = group * G;
-        k_beg = chunk * rows_per_chunk;
-        rows = min(K, k_beg + rows_per_chunk) - k_beg;
+        for (int m = 0; m < G; ++m) any = any || (slot0 + m < n_slots && slot_active(sa, slot0 + m));
         const int64_t E0 = (src.idx64 ? src.idx64[slot0] : (src.idx32 ? (int64_t)src.idx32[slot0] * src.mul : 0)) + src.off;
-        a = (int)(E0 & 3);
-        return src.base + (E0 - a) + (int64_t)k_beg * N;       // 16B-aligned start of the chunk's aligned rows
+        pE0[g] = E0;
+        pb0[g] = any ? (int)(E0 / N / GU_BLK) : INT_MAX;
+        pb1[g] = any ? (int)((E0 + (int64_t)K * N - 1) / N / GU_BLK) : -1;
+    }
+    __syncthreads();
+    // ---- step 2: rank sort by (first block, group) ----
+    for (int g = tid; g < n_groups; g += GB_THREADS) {
+        const int key = pb0[g];
+        int r = 0;
+        for (int h = 0; h < n_groups; ++h) {
+            const int kh = pb0[h];
+            r += (kh < key) || (kh == key && h < g);
+        }
+        psort[r] = g;
+    }
+    __syncthreads();
+    // ---- step 3 (warp 0): blocks each sorted entry adds to the union, and their prefix sum = item numbering ----
+    if (warp == 0) {
+        int carry_max = -1, carry_sum = 0;
+        for (int i0 = 0; i0 < n_groups; i0 += 32) {
+            const int i = i0 + lane;
+            const int g = i < n_groups ? psort[i] : 0;
+            const int b0 = i < n_groups ? pb0[g] : INT_MAX, b1 = i < n_groups ? pb1[g] : -1;
+            int mx = b1;                                  // inclusive max scan of the last blocks
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int o = __shfl_up_sync(0xffffffffu, mx, d);
+                if (lane >= d) mx = max(mx, o);
+            }
+            int before = __shfl_up_sync(0xffffffffu, mx, 1);
+            if (lane == 0) before = -1;
+            before = max(before, carry_max);
+            const int start = max(b0, before + 1);
+            const int add = (b0 != INT_MAX && b1 >= start) ? b1 - start + 1 : 0;
+            int sum = add;                                // inclusive sum scan
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int o = __shfl_up_sync(0xffffffffu, sum, d);
+                if (lane >= d) sum += o;
+            }
+            if (i < n_groups) { pstart[i] = start; ppre[i] = carry_sum + sum - add; }
+            carry_sum += __shfl_sync(0xffffffffu, sum, 31);
+            carry_max = max(carry_max, __shfl_sync(0xffffffffu, mx, 31));
+        }
+        if (lane == 0) s_items = carry_sum;
+    }
+    __syncthreads();
+    const int n_items = s_items;
+    auto item_block = [&](int q) {                     // sorted entry i with ppre[i] <= q < ppre[i] + added_i (the last such)
+        int lo = 0, hi = n_groups;                     // first index with ppre > q
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (ppre[mid] <= q) lo = mid + 1; else hi = mid;
+        }
+        return pstart[lo - 1] + (q - ppre[lo - 1]);
+    };
+    // rows [row0, row0 + n_elem / N) of the table cover the pass: from the first covered row of block b to the last,
+    // ending at the 16-byte-rounded end of the furthest slice (never past the table)
+    auto pass_range = [&](int b, const int* gl, int ng, int64_t& row0, int& n_elem) {
+        int64_t r_first = INT64_MAX, e_last = 0;
+        for (int i = 0; i < ng; ++i) {
+            const int64_t E0 = pE0[gl[i]];
+            r_first = min(r_first, E0 / N);
+            e_last = max(e_last, (E0 + (int64_t)K * N + 3) & ~(int64_t)3);
+        }
+        const int64_t blk0 = (int64_t)b * GU_BLK;
+        row0 = max(r_first, blk0);
+        const int64_t e_end = min(e_last, (blk0 + GU_BLK) * N);
+        n_elem = (int)(e_end - row0 * N);
     };
 
     if (warp == GB_CONSUMERS / 32) {
-        // ===================== producer warp (one elected lane) =====================
-        if (lane == 0) {
-            // L2 prefetch cursor: runs pf_dist stage-blocks ahead of the copy cursor (across work-item boundaries), so the
-            // HBM latency is covered by L2 and the shared-memory ring only has to cover the L2 -> SM latency.  That lets a
-            // shallow ring (1 CTA/SM, <= 64 KB) stream at HBM rate and leaves shared memory for a co-resident conv CTA.
-            int p_item = blockIdx.x - gridDim.x, p_r0 = 0, p_rows = 0;
-            const float* p_base = nullptr;
-            auto p_next_item = [&]() {
-                do { p_item += gridDim.x; } while (p_item < n_items && !item_active(p_item));
-                if (p_item < n_items) { int kb, a_; p_base = item_base(p_item, kb, p_rows, a_); p_r0 = 0; }
-            };
-            auto p_step = [&]() {                                // prefetch the cursor's block, then advance it
-                if (p_item >= n_items) return;
-                bulk_prefetch_l2(p_base + (int64_t)p_r0 * N, (uint32_t)min(RB, p_rows - p_r0) * N * 4);
-                p_r0 += RB;
-                if (p_r0 >= p_rows) p_next_item();
-            };
-            if (pf_dist > 0) {
-                p_next_item();
-                for (int d = 0; d < pf_dist; ++d) p_step();
-            }
-            uint32_t it = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                if (!item_active(item)) continue;
-                int k_beg, rows, a;
-                const float* base = item_base(item, k_beg, rows, a);
-                for (int r0 = 0; r0 < rows; r0 += RB, ++it) {
-                    if (pf_dist > 0) p_step();
-                    const int s = it % n_stages;
-                    mbar_wait(&empty_bar[s], ((it / n_stages) & 1) ^ 1);
-                    const uint32_t bytes = (uint32_t)min(RB, rows - r0) * N * 4;
-                    mbar_arrive_expect_tx(&full_bar[s], bytes);
-                    bulk_g2s(stage_base + (size_t)s * (GB_STAGE_BYTES / 4), base + (int64_t)r0 * N, bytes, &full_bar[s]);
+        // ===================== producer warp =====================
+        uint32_t it = 0;
+        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+            const int b = item_block(item);
+            int total = CAP;
+            for (int first = 0; first < total; first += CAP) {
+                total = gu_cover(pb0, pb1, n_groups, b, first, CAP, cov_p, lane);
+                int64_t row0;
+                int n_elem;
+                pass_range(b, cov_p, min(CAP, total - first), row0, n_elem);
+                const float* gsrc = src.base + row0 * N;
+                for (int e0 = 0; e0 < n_elem; e0 += RB * N, ++it) {
+                    if (lane == 0) {
+                        const int s = it % n_stages;
+                        mbar_wait(&empty_bar[s], ((it / n_stages) & 1) ^ 1);
+                        const uint32_t bytes = (uint32_t)min(RB * N, n_elem - e0) * 4;
+                        mbar_arrive_expect_tx(&full_bar[s], bytes);
+                        bulk_g2s(stage_base + (size_t)s * (GB_STAGE_BYTES / 4), gsrc + e0, bytes, &full_bar[s]);
+                    }
                 }
+                __syncwarp();                          // cov_p is rewritten by the next pass
             }
         }
         return;
@@ -129,219 +216,171 @@ gemv_bulk_kernel(SlotArgs sa, GemvSrc src, const float* __restrict__ X, int64_t 
     pdl_wait();
     const int t = tid % NQ, rw = tid / NQ;
     const int red_ld = N + 4;
+    float* red = xs;                                   // [RW][GU_VB][N + 4], after the last stage of a pass
     uint32_t it = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        if (!item_active(item)) continue;
-        const int group = item / n_chunks, chunk = item % n_chunks;
-        const int slot0 = group * G;
-        int k_beg, rows, a;
-        const float* base = item_base(item, k_beg, rows, a);
-
-        float tv[GB_FOLD_O][GB_FOLD_S];
-        if (tpart) {
-#pragma unroll
-            for (int o = 0; o < GB_FOLD_O; ++o) {
-                const int i = tid + o * GB_CONSUMERS;
-                const int g = i / N, n = i - g * N;
-                const bool ok = i < G * N && slot0 + g < n_slots;
-#pragma unroll
-                for (int k = 0; k < GB_FOLD_S; ++k) {
-                    const int j = chunk + k * n_chunks;
-                    // volatile asm: the load is issued HERE (the compiler otherwise sinks it to its use after the streaming
-                    // loop and exposes one L2 round trip per item: measured +8 us per GEMV launch)
-                    float v = 0.0f;
-                    if (ok && j < t_split)
-                        asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(v) : "l"(tpart + ((int64_t)j * n_slots + slot0 + g) * N + n) : "memory");
-                    tv[o][k] = v;
+        const int b = item_block(item);
+        int total = CAP;
+        for (int first = 0; first < total; first += CAP) {
+            if (warp == 0) {
+                const int tot = gu_cover(pb0, pb1, n_groups, b, first, CAP, cov_c, lane);
+                if (lane == 0) {
+                    const int ng = min(CAP, tot - first);
+                    int64_t row0;
+                    int n_elem;
+                    pass_range(b, cov_c, ng, row0, n_elem);
+                    s_total = tot;
+                    s_row0 = (int)(row0 - (int64_t)b * GU_BLK);     // block-relative
+                    s_nelem = n_elem;
+                    for (int i = 0; i < ng; ++i) rho_c[i] = (int)(pE0[cov_c[i]] % N);
                 }
             }
-        }
-        // stage x_g[k_beg-1 .. k_beg+rows) (the previous item's readers are past their last xs read: barrier C below)
-        for (int i = tid; i < G * (rows + 1); i += GB_CONSUMERS) {
-            const int g = i / (rows + 1), r = i % (rows + 1);
-            const int k = k_beg - 1 + r;
-            xs[g][r] = (k >= 0) ? X[(int64_t)(slot0 + g) * x_slot_stride + k] : 0.0f;
-        }
-        named_bar_sync(1, GB_CONSUMERS);                                   // barrier A
+            named_bar_sync(1, GB_CONSUMERS);                               // barrier A: pass plan
+            total = s_total;
+            const int ng = min(CAP, total - first), nv = ng * G;
+            const int lrow0 = s_row0, n_elem = s_nelem;
+            // stage x_v over block rows -1 .. XS_LD-2: xs[v][L + 1] = x_v[k], k = row - R_g, zero outside [0, K)
+            for (int i = tid; i < nv * XS_LD; i += GB_CONSUMERS) {
+                const int v = i / XS_LD, L = i - v * XS_LD - 1;
+                const int g = cov_c[v / G], slot = g * G + v % G;
+                const int64_t k = (int64_t)b * GU_BLK + L - pE0[g] / N;
+                xs[v * XS_LD + L + 1] = (k >= 0 && k < K && slot < n_slots) ? X[(int64_t)slot * x_slot_stride + k] : 0.0f;
+            }
+            named_bar_sync(1, GB_CONSUMERS);                               // barrier B: xs staged
 
-        float acc[G][4], wrap[G][4];
+            float acc[GU_VEC][4];
 #pragma unroll
-        for (int g = 0; g < G; ++g)
+            for (int v = 0; v < GU_VEC; ++v)
 #pragma unroll
-            for (int c = 0; c < 4; ++c) acc[g][c] = wrap[g][c] = 0.0f;
-        const bool do_wrap = (t == 0) && (a != 0);
+                for (int c = 0; c < 4; ++c) acc[v][c] = 0.0f;
 
-        for (int r0 = 0; r0 < rows; r0 += RB, ++it) {
-            const int s = it % n_stages;
-            const int nr = min(RB, rows - r0);
-            const int rl0 = rw * GB_RPR;                 // this reader's first row inside the stage (contiguous rows)
-            // x multipliers: xm[g][j] = x[r0+rl0+j] (row itself), xm[g][-1 -> index 0] = x[r0+rl0-1] (wrap of the first row)
-            float xm[G][GB_RPR + 1];
+            for (int e0 = 0; e0 < n_elem; e0 += RB * N, ++it) {
+                const int s = it % n_stages;
+                const int stage_elems = min(RB * N, n_elem - e0);
+                const int rl0 = rw * GB_RPR;           // this reader's first row inside the stage (contiguous rows)
+                const int xb0 = lrow0 + e0 / N + rl0;  // xs index of x[k - 1] for the reader's first row
+                mbar_wait(&full_bar[s], (it / n_stages) & 1);
+                // explicit ld.shared (a C++ pointer into the re-aligned dynamic smem compiles to generic LD.E)
+                const uint32_t rows_a = wg::smem_u32(stage_base) + s * GB_STAGE_BYTES + (rl0 * NQ + t) * 16;
+                float4 w[GB_RPR];
 #pragma unroll
-            for (int g = 0; g < G; ++g)
+                for (int j = 0; j < GB_RPR; ++j)       // columns past the streamed end (last row of the pass) are zero
+                    w[j] = ((rl0 + j) * N + 4 * t < stage_elems) ? wg::lds128(rows_a + j * NQ * 16) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-                for (int j = 0; j <= GB_RPR; ++j) xm[g][j] = xs[g][r0 + rl0 + j];        // xs index = 1 + (row - 1)
-            mbar_wait(&full_bar[s], (it / n_stages) & 1);
-            // explicit ld.shared (a C++ pointer into the re-aligned dynamic smem compiles to generic LD.E)
-            const uint32_t rows_a = wg::smem_u32(stage_base) + s * GB_STAGE_BYTES + (rl0 * NQ + t) * 16;
-            if (nr == RB) {
-                float4 v[GB_RPR];
+                for (int gi = 0; gi < CAP; ++gi) {
+                    if (gi < ng) {
+                        const int rho = rho_c[gi];     // components c < rho carry row k - 1
+                        const bool p0 = 4 * t < rho, p1 = 4 * t + 1 < rho, p2 = 4 * t + 2 < rho, p3 = 4 * t + 3 < rho;
 #pragma unroll
-                for (int j = 0; j < GB_RPR; ++j) v[j] = wg::lds128(rows_a + j * NQ * 16);
+                        for (int m = 0; m < G; ++m) {
+                            const int v = gi * G + m;
+                            float xm[GB_RPR + 1];
 #pragma unroll
-                for (int j = 0; j < GB_RPR; ++j)
+                            for (int j = 0; j <= GB_RPR; ++j) xm[j] = xs[v * XS_LD + xb0 + j];
 #pragma unroll
-                    for (int g = 0; g < G; ++g) {
-                        acc[g][0] = fmaf(xm[g][j + 1], v[j].x, acc[g][0]);
-                        acc[g][1] = fmaf(xm[g][j + 1], v[j].y, acc[g][1]);
-                        acc[g][2] = fmaf(xm[g][j + 1], v[j].z, acc[g][2]);
-                        acc[g][3] = fmaf(xm[g][j + 1], v[j].w, acc[g][3]);
-                    }
-                if (do_wrap) {
-#pragma unroll
-                    for (int j = 0; j < GB_RPR; ++j)
-#pragma unroll
-                        for (int g = 0; g < G; ++g) {     // aligned row r carries weight row r-1 in its columns q < a
-                            const float xp = (r0 + rl0 + j >= 1) ? xm[g][j] : 0.0f;
-                            wrap[g][0] = fmaf(xp, v[j].x, wrap[g][0]);
-                            wrap[g][1] = fmaf(xp, v[j].y, wrap[g][1]);
-                            wrap[g][2] = fmaf(xp, v[j].z, wrap[g][2]);
-                            wrap[g][3] = fmaf(xp, v[j].w, wrap[g][3]);
-                        }
-                }
-            } else {
-                for (int j = 0; j < GB_RPR; ++j) {
-                    if (rl0 + j < nr) {
-                        const float4 v = wg::lds128(rows_a + j * NQ * 16);
-#pragma unroll
-                        for (int g = 0; g < G; ++g) {
-                            acc[g][0] = fmaf(xm[g][j + 1], v.x, acc[g][0]);
-                            acc[g][1] = fmaf(xm[g][j + 1], v.y, acc[g][1]);
-                            acc[g][2] = fmaf(xm[g][j + 1], v.z, acc[g][2]);
-                            acc[g][3] = fmaf(xm[g][j + 1], v.w, acc[g][3]);
-                            if (do_wrap && (r0 + rl0 + j >= 1)) {
-                                wrap[g][0] = fmaf(xm[g][j], v.x, wrap[g][0]);
-                                wrap[g][1] = fmaf(xm[g][j], v.y, wrap[g][1]);
-                                wrap[g][2] = fmaf(xm[g][j], v.z, wrap[g][2]);
-                                wrap[g][3] = fmaf(xm[g][j], v.w, wrap[g][3]);
+                            for (int j = 0; j < GB_RPR; ++j) {
+                                acc[v][0] = fmaf(p0 ? xm[j] : xm[j + 1], w[j].x, acc[v][0]);
+                                acc[v][1] = fmaf(p1 ? xm[j] : xm[j + 1], w[j].y, acc[v][1]);
+                                acc[v][2] = fmaf(p2 ? xm[j] : xm[j + 1], w[j].z, acc[v][2]);
+                                acc[v][3] = fmaf(p3 ? xm[j] : xm[j + 1], w[j].w, acc[v][3]);
                             }
                         }
                     }
                 }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[s]);           // this warp is done reading stage s
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[s]);           // this warp is done reading stage s
-        }
-        // the chunk's last weight row (k = rows-1) wraps into aligned row `rows`, the first row of the NEXT chunk:
-        // one 16-byte load per item
-        if (do_wrap && rw == 0) {
-            const float4 v = ldg_stream_f4(base + (int64_t)rows * N);
+            // cross-reader reduction in fixed order, GU_VB vectors per round (red aliases xs: wait for every reader)
+            for (int vb0 = 0; vb0 < nv; vb0 += GU_VB) {
+                named_bar_sync(1, GB_CONSUMERS);                           // barrier C: xs / red free
 #pragma unroll
-            for (int g = 0; g < G; ++g) {
-                const float x = xs[g][rows];                      // x[k_beg + rows - 1]
-                wrap[g][0] = fmaf(x, v.x, wrap[g][0]);
-                wrap[g][1] = fmaf(x, v.y, wrap[g][1]);
-                wrap[g][2] = fmaf(x, v.z, wrap[g][2]);
-                wrap[g][3] = fmaf(x, v.w, wrap[g][3]);
-            }
-        }
-        // cross-reader reduction in fixed order, then this item's partial [G][N]
+                for (int v = 0; v < GU_VEC; ++v) {
+                    if (v >= vb0 && v < vb0 + GU_VB && v < nv) {
+                        const int rho = rho_c[v / G];
+                        float* row = red + (rw * GU_VB + (v - vb0)) * red_ld;
 #pragma unroll
-        for (int g = 0; g < G; ++g) {
-            float* row = red + (rw * G + g) * red_ld;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const int q = 4 * t + c;
-                if (q >= a) row[q - a] = acc[g][c];
-            }
-            if (t == 0) {
-#pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    if (c < a) row[N + c - a] = wrap[g][c];
-            }
-        }
-        named_bar_sync(1, GB_CONSUMERS);                                   // barrier B
-        float* out = part + ((int64_t)group * n_chunks + chunk) * G * N;
-        if (tpart) {
-#pragma unroll
-            for (int o = 0; o < GB_FOLD_O; ++o) {
-                const int i = tid + o * GB_CONSUMERS;
-                if (i < G * N) {
-                    const int g = i / N, n = i - g * N;
+                        for (int c = 0; c < 4; ++c) {
+                            const int n = 4 * t + c - rho;
+                            row[n < 0 ? n + N : n] = acc[v][c];
+                        }
+                    }
+                }
+                named_bar_sync(1, GB_CONSUMERS);                           // barrier D
+                for (int i = tid; i < GU_VB * N; i += GB_CONSUMERS) {
+                    const int vl = i / N, n = i - vl * N, v = vb0 + vl;
+                    if (v >= nv) break;
+                    const int g = cov_c[v / G], m = v % G, slot = g * G + m;
+                    const int piece = b - pb0[g];
                     float sum = 0.0f;
-                    for (int w = 0; w < RW; ++w) sum += red[(w * G + g) * red_ld + n];
-                    float ts = tv[o][0];
-#pragma unroll
-                    for (int k = 1; k < GB_FOLD_S; ++k) ts += tv[o][k];
-                    out[i] = fmaf(slot0 + g < n_slots ? sa.scale[slot0 + g] : 0.0f, sum, ts);
+                    for (int w2 = 0; w2 < RW; ++w2) sum += red[(w2 * GU_VB + vl) * red_ld + n];
+                    if (tpart) {
+                        float ts = 0.0f;
+                        if (slot < n_slots)
+                            for (int j = piece; j < t_split; j += n_pieces) ts += tpart[((int64_t)j * n_slots + slot) * N + n];
+                        sum = fmaf(slot < n_slots ? sa.scale[slot] : 0.0f, sum, ts);
+                    }
+                    part[(((int64_t)g * n_pieces + piece) * G + m) * N + n] = sum;
                 }
             }
-        } else {
-            for (int i = tid; i < G * N; i += GB_CONSUMERS) {
-                const int g = i / N, n = i % N;
-                float sum = 0.0f;
-                for (int w = 0; w < RW; ++w) sum += red[(w * G + g) * red_ld + n];
-                out[i] = sum;
+            // pieces past a group's last block: zero (+ the folded theta partials), written with the group's last block
+            for (int gi = 0; gi < ng; ++gi) {
+                const int g = cov_c[gi];
+                if (pb1[g] != b) continue;
+                for (int piece = b - pb0[g] + 1; piece < n_pieces; ++piece)
+                    for (int i = tid; i < G * N; i += GB_CONSUMERS) {
+                        const int m = i / N, n = i - m * N, slot = g * G + m;
+                        float ts = 0.0f;
+                        if (tpart && slot < n_slots)
+                            for (int j = piece; j < t_split; j += n_pieces) ts += tpart[((int64_t)j * n_slots + slot) * N + n];
+                        part[(((int64_t)g * n_pieces + piece) * G + m) * N + n] = ts;
+                    }
             }
+            named_bar_sync(1, GB_CONSUMERS);                               // barrier E: red[], xs[], cov_c[] reusable
         }
-        named_bar_sync(1, GB_CONSUMERS);                                   // barrier C: red[] and xs[] reusable
     }
 }
 
-bool dne_gemv_bulk_can_fold(int G, int N, int n_chunks, int n_split) {
-    return G * N <= GB_FOLD_O * GB_CONSUMERS && n_split >= 1 && n_split <= GB_FOLD_S * n_chunks;
-}
+int dne_gemv_pieces(int K) { return (K + 1 + GU_BLK - 1) / GU_BLK + 1; }
 
-int dne_launch_gemv_bulk(const SlotArgs& sa, const GemvSrc& src, int G, const float* X, int64_t x_slot_stride, int K,
-                         int N, int rows_per_chunk, int n_chunks, int n_slots, float* part, int sm_count,
-                         cudaStream_t st, const float* fold_theta, int fold_n_split) {
-    if (fold_theta && !dne_gemv_bulk_can_fold(G, N, n_chunks, fold_n_split)) return DNE_ERR_UNSUP;
-    // shape cover: 4 | N, N/4 divides 256, one stage = GB_RPR rows per reader
-    if (N % 4 != 0 || N * 4 > GB_STAGE_BYTES || (GB_CONSUMERS % (N / 4)) != 0) return DNE_ERR_UNSUP;
+int dne_launch_gemv_union(const SlotArgs& sa, const GemvSrc& src, int G, const float* X, int64_t x_slot_stride, int K,
+                          int N, int n_pieces, int n_slots, float* part, int sm_count, cudaStream_t st,
+                          const float* fold_theta, int fold_n_split) {
+    // shape cover: 4 | N, N/4 divides 256, one stage = GB_RPR rows per reader, at most GU_BLK / 4 rows per stage
+    if (N % 4 != 0 || N < GU_MIN_N || N * 4 > GB_STAGE_BYTES || (GB_CONSUMERS % (N / 4)) != 0) return DNE_ERR_UNSUP;
     const int RW = GB_CONSUMERS / (N / 4);
-    if (GB_RPR * RW * N * 4 != GB_STAGE_BYTES || rows_per_chunk > GB_MAX_ROWS) return DNE_ERR_UNSUP;
+    if (GB_RPR * RW * N * 4 != GB_STAGE_BYTES || n_pieces != dne_gemv_pieces(K) || (G != 1 && G != 2)) return DNE_ERR_UNSUP;
     const int n_groups = (n_slots + G - 1) / G;
-    const int n_stages = g_dne_gemv_stages;
-    const size_t smem = (size_t)n_stages * GB_STAGE_BYTES + (size_t)RW * G * (N + 4) * sizeof(float) + 128;
-    const int n_items = n_groups * n_chunks;
-    int grid = g_dne_gemv_ctas_per_sm * sm_count;
-    if (g_dne_gemv_grid > 0 && grid > g_dne_gemv_grid) grid = g_dne_gemv_grid;
-    if (grid > n_items) grid = n_items;
-    else if (g_dne_gemv_balance) {
-        // the items are dealt round-robin: pick the grid size in [7/8 * grid, grid] that leaves the fewest idle item slots in
-        // the last round (62 pairs x 32 chunks on 296 CTAs: 7 rounds with 88 idle slots; on 284 CTAs: 4 idle slots)
-        int best = grid;
-        long best_waste = (long)((n_items + grid - 1) / grid) * grid - n_items;
-        for (int g = grid - 1; g >= grid - grid / 8 && best_waste > 0; --g) {
-            const long waste = (long)((n_items + g - 1) / g) * g - n_items;
-            if (waste < best_waste) { best_waste = waste; best = g; }
-        }
-        grid = best;
+    if (n_groups <= 0) return 0;
+    // shared memory: static (xs + barriers) + ring + plan; as many ring stages as fit next to the chosen CTAs per SM
+    const size_t static_smem = (size_t)GU_XS_FLOATS * 4 + 1024;
+    const size_t plan = (size_t)n_groups * GU_PLAN_BYTES_PER_GROUP + 128;
+    const size_t per_sm = 227 * 1024;
+    int cps = g_dne_gemv_ctas_per_sm, n_stages = 0;
+    for (; cps >= 1; --cps) {
+        const size_t budget = per_sm / cps - 1024;
+        n_stages = budget > static_smem + plan ? (int)((budget - static_smem - plan) / GB_STAGE_BYTES) : 0;
+        if (n_stages > g_dne_gemv_stages) n_stages = g_dne_gemv_stages;
+        if (n_stages >= 2) break;
     }
+    if (cps < 1) return DNE_ERR_UNSUP;
+    const size_t smem = (size_t)n_stages * GB_STAGE_BYTES + plan;
+    int grid = cps * sm_count;
+    if (g_dne_gemv_grid > 0 && grid > g_dne_gemv_grid) grid = g_dne_gemv_grid;
     int dev = 0;
     cudaGetDevice(&dev);
     static bool attr_done_dev[64][3] = {};                        // per device: one process may drive several GPUs
     bool* attr_done = attr_done_dev[dev < 64 ? dev : 63];
-    if (G == 2) {
-        if (!attr_done[2]) {
-            cudaFuncSetAttribute(gemv_bulk_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            if (cudaFuncSetAttribute(gemv_bulk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (GB_STAGES * 16 + 12) * 1024) != cudaSuccess)
+    auto launch = [&](auto kern) -> int {
+        if (!attr_done[G]) {
+            cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_sm - static_smem - 1024)) != cudaSuccess)
                 return DNE_ERR_CUDA;
-            attr_done[2] = true;
+            attr_done[G] = true;
         }
-        if (dne_launch_chain(gemv_bulk_kernel<2>, dim3(grid), dim3(GB_THREADS), smem, st, true, sa, src, X, x_slot_stride, K, N,
-                             rows_per_chunk, n_chunks, n_groups, part, n_stages, g_dne_gemv_prefetch, fold_theta, fold_n_split, n_slots) != cudaSuccess)
+        if (dne_launch_chain(kern, dim3(grid), dim3(GB_THREADS), smem, st, true, sa, src, X, x_slot_stride, K, N, n_pieces,
+                             n_groups, n_slots, part, n_stages, fold_theta, fold_theta ? fold_n_split : 0) != cudaSuccess)
             return DNE_ERR_CUDA;
-    } else {
-        if (!attr_done[1]) {
-            cudaFuncSetAttribute(gemv_bulk_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            if (cudaFuncSetAttribute(gemv_bulk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (GB_STAGES * 16 + 12) * 1024) != cudaSuccess)
-                return DNE_ERR_CUDA;
-            attr_done[1] = true;
-        }
-        if (dne_launch_chain(gemv_bulk_kernel<1>, dim3(grid), dim3(GB_THREADS), smem, st, true, sa, src, X, x_slot_stride, K, N,
-                             rows_per_chunk, n_chunks, n_groups, part, n_stages, g_dne_gemv_prefetch, fold_theta, fold_n_split, n_slots) != cudaSuccess)
-            return DNE_ERR_CUDA;
-    }
-    return 0;
+        return 0;
+    };
+    return G == 2 ? launch(gemv_union_kernel<2>) : launch(gemv_union_kernel<1>);
 }

@@ -104,10 +104,10 @@ long long   dne_launch_count(int reset);
  *   "pdl" = 1 (default): the tick's kernels are chained by programmatic dependent launch (griddepcontrol).
  *   "chain_ticks" = 0 (default): 1 = the tick's first convolution is a dependent launch too; only valid when the stream's
  *               previous kernel is the previous tick's last kernel (nothing that writes theta / the noise table / the slot table).
- *   "gemv_balance" = 1 (default): the GEMV grid size is chosen to balance the round-robin deal of work items.
- *   "gemv_bulk" = 1 (default): noise GEMV through the cp.async.bulk shared-memory ring; 0 = plain-LDG kernel.
- *   "gemv_ctas_per_sm" = 1|2 (default 2), "gemv_stages" = 2..8 (default 6), "gemv_grid" (default 0 = no cap),
- *   "gemv_chunk_kb" (work-item size), "gemv_prefetch" = 0..256 (default 0; L2 prefetch distance, measured slower). */
+ *   "gemv_bulk" = 1 (default): the dense layers' GEMV streams the union of the slot table's slices once, through the
+ *               cp.async.bulk shared-memory ring; 0 = plain-LDG kernel, one slice per group (the parity referee).
+ *   "gemv_ctas_per_sm" = 1|2 (default 2), "gemv_stages" = 2..8 (default 5, upper bound on the ring depth that fits),
+ *   "gemv_grid" (default 0 = no cap). */
 int         dne_set_option(const char* name, int value);
 int         dne_profile_enable(dne_ctx* ctx, int on, int capacity);
 int         dne_profile_read(dne_ctx* ctx, int* n_launches, double* total_ms);

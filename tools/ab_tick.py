@@ -18,7 +18,7 @@ for v in os.environ.get("VARIANTS", "base:").split(";"):
     name, _, spec = v.partition(":")
     variants.append((name, [kv.split("=") for kv in spec.split(",") if kv]))
 keys = sorted({k for _, kv in variants for k, _ in kv})
-defaults = {"chain_ticks": 0, "fold_theta": 1, "gemv_balance": 1, "pdl": 1, "fuse_head": 1, "theta_tma": 1, "gemv_stages": 6, "gemv_ctas_per_sm": 2, "gemv_grid": 0}
+defaults = {"chain_ticks": 0, "fold_theta": 1, "pdl": 1, "fuse_head": 1, "theta_tma": 1, "gemv_stages": 5, "gemv_ctas_per_sm": 2, "gemv_grid": 0}
 ROUNDS, TICKS = int(os.environ.get("ROUNDS", 7)), int(os.environ.get("TICKS", 150))
 for slots in [int(x) for x in os.environ.get("SLOTS_LIST", "124,256").split(",")]:
     pidx = rs.randint(0, count - P + 1, size=slots // 2).astype(np.int64)

@@ -16,10 +16,9 @@ L = F.lib()
 net_ref = C.byref(net.desc)
 R = 4
 
-def run(total, NS, gemv_ctas, mode, stages=6, pf=0, ticks=300):
+def run(total, NS, gemv_ctas, mode, stages=5, ticks=300):
     F.check(L.dne_set_option(b"gemv_ctas_per_sm", gemv_ctas))
     F.check(L.dne_set_option(b"gemv_stages", stages))
-    F.check(L.dne_set_option(b"gemv_prefetch", pf))
     part = (total // NS) // 2 * 2
     sfs = [SlotForward(ctx, net, part) for _ in range(NS)]
     for sf in sfs:
@@ -51,13 +50,11 @@ def run(total, NS, gemv_ctas, mode, stages=6, pf=0, ticks=300):
     a.record(); loop(ticks); b.record(); torch.cuda.synchronize()
     L.dne_set_phase_events(ctx.handle, None, None, 0)
     us = a.elapsed_time(b) * 1e3 / ticks
-    print(f"slots={NS * part:4d} tables={NS} gemv_ctas/SM={gemv_ctas} stages={stages} l2_prefetch={pf:2d} phase_mode={mode:2d}: tick {us:7.1f} us  -> {NS * part / us * 1e6 / 1e3:7.1f}K env-steps/s", flush=True)
+    print(f"slots={NS * part:4d} tables={NS} gemv_ctas/SM={gemv_ctas} stages={stages} phase_mode={mode:2d}: tick {us:7.1f} us  -> {NS * part / us * 1e6 / 1e3:7.1f}K env-steps/s", flush=True)
 
 CFGS = eval(os.environ["SWEEP"]) if os.environ.get("SWEEP") else None
-for cfg in CFGS or [(256, 1, 2, -1, 6, 0), (256, 1, 2, -1, 6, 16), (256, 1, 2, -1, 3, 16), (256, 1, 1, -1, 6, 0), (256, 1, 1, -1, 8, 0),
-            (256, 1, 1, -1, 6, 16), (256, 1, 1, -1, 4, 16), (256, 1, 1, -1, 4, 32), (256, 1, 1, -1, 3, 32), (256, 1, 1, -1, 3, 64),
-            (512, 2, 2, -1, 6, 0), (512, 2, 1, 1, 6, 16), (512, 2, 1, 1, 4, 32), (512, 2, 1, 1, 3, 32), (512, 2, 1, -1, 4, 32),
-            (512, 2, 1, -1, 3, 32), (512, 4, 1, 1, 4, 32), (512, 2, 2, -1, 3, 16)]:
+for cfg in CFGS or [(256, 1, 2, -1, 5), (256, 1, 1, -1, 8), (256, 1, 1, -1, 4), (512, 2, 2, -1, 5), (512, 2, 1, 1, 4),
+            (512, 4, 1, 1, 4), (512, 2, 2, -1, 3)]:
     try:
         run(*cfg)
     except Exception as e:

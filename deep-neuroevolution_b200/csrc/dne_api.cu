@@ -455,6 +455,32 @@ extern "C" int dne_perturb_forward_conv(dne_ctx* ctx, const dne_net_desc* net, c
                         nullptr, nullptr, d_vbn, d_actions, d_logits, d_ws, ws_bytes, stream);
 }
 
+extern "C" int dne_cartpole_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                                     const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                     int n_members, const double* d_init_state, int max_steps, float* d_returns,
+                                     int32_t* d_lengths, double* d_final_state, void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_lengths, "null pointer");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1, "max_steps < 1");
+    const char* why = "";
+    if (!dne_cartpole_net_supported(net, &why)) {
+        dne_set_error("dne_cartpole_episodes: net not supported by the episode kernel: %s", why);
+        return DNE_ERR_UNSUP;
+    }
+    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
+    if (n_members == 0) return DNE_OK;
+    const int rc = dne_launch_cartpole_episodes(net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx, n_members,
+                                                d_init_state, max_steps, d_returns, d_lengths, d_final_state,
+                                                (cudaStream_t)stream);
+    if (rc) {
+        dne_set_error("dne_cartpole_episodes: launch setup failed (%d)", rc);
+        return rc;
+    }
+    DNE_LAUNCH_CHECK();
+    return DNE_OK;
+}
+
 extern "C" int dne_perturb_forward_mlp(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
                                        const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
                                        const uint8_t* d_active, int n_slots, int paired, const float* d_obs,

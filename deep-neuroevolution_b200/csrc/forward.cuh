@@ -94,6 +94,12 @@ int dne_launch_dense_layer(const dne_ctx* ctx, const SlotArgs& sa, const dne_lay
 void dne_launch_ob_norm(const float* obs, const float* mean, const float* stdv, int64_t total, int dim, float* out,
                         cudaStream_t st);
 
+// episode_kernels.cu: whole CartPole-v1 episodes on the device (dne_cartpole_episodes)
+bool dne_cartpole_net_supported(const dne_net_desc* net, const char** why);
+int dne_launch_cartpole_episodes(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,
+                                 const float* scale, const int32_t* theta_idx, int n_members, const double* init_state,
+                                 int max_steps, float* returns, int32_t* lengths, double* final_state, cudaStream_t st);
+
 int dne_launch_theta_gemm_tc(const float* X, int M, int K, int N, const float* W, int k_per_split, int n_split,
                              float* part, cudaStream_t st);
 

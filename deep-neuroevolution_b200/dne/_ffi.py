@@ -51,6 +51,7 @@ _SIGS = {
     "dne_perturb_forward_mlp": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P,
                                 C.c_size_t, _P],
     "dne_ob_stat_accumulate": [_P, C.c_int, _P, C.c_int, _P, _P, _P],
+    "dne_cartpole_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P],
     "dne_theta_prepare": [_P, C.POINTER(NetDesc), _P, C.c_int, _P, C.c_size_t, _P],
     "dne_theta_forget": [_P, _P],
     "dne_vbn_ws_bytes": [C.POINTER(NetDesc), C.c_int, C.c_int, C.POINTER(C.c_size_t)],

@@ -9,7 +9,8 @@ Step`` over a batch of ALE instances (gpu_implementation/gym_tensorflow/tf_env.c
 ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so the environment shipped
 here is the synthetic Frostbite-shaped stub the measurement plan names (SURVEY.md 8d): i.i.d. uint8 84x84x4
 observations from a fixed pool, rewards 10*Bernoulli(0.05), fixed or ragged episode lengths.  A real emulator
-plugs in by subclassing ``BatchEnv``.
+plugs in by subclassing ``BatchEnv``.  One real task needs no emulator: CartPole-v1 (``CartPoleEnv``), whose episodes run
+whole on the device (``dne.rollout.EpisodeKernelRunner``).
 """
 from __future__ import annotations
 
@@ -200,8 +201,8 @@ class SyntheticVectorEnv(BatchEnv):
 def make_env(env_id: str, n_slots: int, seed: int = 0, episode_len=None, allow_synthetic: bool = False, **kw) -> BatchEnv:
     """``gym.make(exp['env_id'])`` (es.py:131) for a whole slot table.
 
-    ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so the only backends here are
-    the synthetic stubs.  They are returned for the explicit ids ``SyntheticAtari*`` / ``SyntheticVector*``; for a REAL id
+    ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so apart from CartPole-v1
+    (``CartPoleEnv``, registered in ``ENV_BACKENDS``) the only backends here are the synthetic stubs.  They are returned for the explicit ids ``SyntheticAtari*`` / ``SyntheticVector*``; for a REAL id
     (``FrostbiteNoFrameskip-v4``, ``Humanoid-v1`` ...) they are returned only when the caller opts in
     (``exp['allow_synthetic_env'] = true`` or ``DNE_ALLOW_SYNTHETIC_ENV=1``), with a loud warning -- a run that silently
     optimised random frames while logging and snapshotting like a real one would be worse than an error.  A real emulator
@@ -231,4 +232,39 @@ def make_env(env_id: str, n_slots: int, seed: int = 0, episode_len=None, allow_s
     return env
 
 
-ENV_BACKENDS = {}        # id prefix -> factory(env_id, n_slots, seed=, episode_len=, **kw) -> BatchEnv (real emulators plug in here)
+class CartPoleEnv(BatchEnv):
+    """gym's CartPole-v1 (classic_control cartpole.py) for a whole population, stepped ON THE DEVICE: whole episodes run in
+    one launch of ``dne_cartpole_episodes`` (``dne.rollout.EpisodeKernelRunner``), so this object only supplies the spaces,
+    the time limit and the reset states.  ``initial_states(k)`` draws k resets ``uniform(-0.05, 0.05, size=4)`` from one
+    ``RandomState(seed)`` stream that continues across calls, as one gym env reset k times in a row would."""
+    device_episodes = True
+
+    def __init__(self, n_slots: int, seed: int = 0):
+        self.n_slots = int(n_slots)
+        high = np.array([2.4 * 2, np.finfo(np.float32).max, (12 * 2 * np.pi / 360) * 2, np.finfo(np.float32).max],
+                        dtype=np.float32)                                        # gym's observation_space bounds
+        self.observation_space = Box(-high, high)
+        self.action_space = Discrete(2)
+        self.max_episode_steps = 500                                             # TimeLimit of CartPole-v1
+        self.rs = np.random.RandomState(seed)
+
+    def initial_states(self, k: int) -> np.ndarray:
+        """float64 [k, 4] reset states (gym ``reset``: ``uniform(low=-0.05, high=0.05, size=(4,))`` per episode)."""
+        return self.rs.uniform(-0.05, 0.05, size=(int(k), 4))
+
+    def _host_stepping(self, *a, **kw):
+        raise NotImplementedError("CartPoleEnv runs whole episodes on the device: use dne.rollout.make_runner "
+                                  "(EpisodeKernelRunner), not the per-tick host reset / step")
+    reset = step = obs_block = get_ram = _host_stepping
+
+
+def _make_cartpole(env_id, n_slots, seed=0, episode_len=None, **kw):
+    if episode_len is not None:
+        raise ValueError("CartPole-v1 has a fixed 500-step time limit; use the episode cutoff of the config instead")
+    return CartPoleEnv(n_slots, seed=seed)
+
+
+ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_len=, **kw) -> BatchEnv (real emulators plug in here)
+    "CartPole-v1": _make_cartpole,
+    "gym.CartPole-v1": _make_cartpole,   # the id of the reference GPU path's configurations/es_gym_config.json
+}

@@ -9,6 +9,8 @@ gpu path gpu_implementation/neuroevolution/models/base.py:165-192):
   ESAtariPolicy  policies.py:319-330      each BN'd layer: weights, biases, BatchNorm/beta, BatchNorm/gamma
   ModelVirtualBN models/batchnorm.py:50-123  Model's layout; layers without bias, 'b' is added AFTER (x-mean)/sqrt(var+eps)
   MujocoPolicy   policies.py:155-162,195  l0..lN dense tanh, 'out' dense (continuous head)
+  SimpleClassifier  models/simple.py:29-34  fc1[ob,16] b fc2[16,16] b out[16,A] b (relu hidden; out std 0.1)
+  LinearClassifier  models/simple.py:23-27  out[ob,A] b
 Kernels are HWIO, activations NHWC, flatten order (h, w, c); conv padding is TF 'SAME'.
 """
 from __future__ import annotations
@@ -146,5 +148,11 @@ def make_net(name: str, num_actions: int = 18, ob_dim: int = 376, hidden: Sequen
         dims = [ob_dim] + list(hidden)
         layers = [_dense(dims[i], dims[i + 1], act=act) for i in range(len(hidden))]
         layers.append(_dense(dims[-1], ac_dim, act=F.ACT_NONE, std=0.01))
+        return _finish(NetSpec(name, layers, F.OB_VECTOR, ob_dim))
+    if name == "SimpleClassifier":               # models/simple.py:29-34: fc1 16 relu, fc2 16 relu, out (std 0.1)
+        layers = [_dense(ob_dim, 16), _dense(16, 16), _dense(16, A, act=F.ACT_NONE, std=0.1)]
+        return _finish(NetSpec(name, layers, F.OB_VECTOR, ob_dim))
+    if name == "LinearClassifier":               # models/simple.py:23-27: out only (default std 1.0)
+        layers = [_dense(ob_dim, A, act=F.ACT_NONE)]
         return _finish(NetSpec(name, layers, F.OB_VECTOR, ob_dim))
     raise KeyError(f"unknown policy/model type {name!r}")

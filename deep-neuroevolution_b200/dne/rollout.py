@@ -11,6 +11,7 @@ Reference behaviour reproduced:
 """
 from __future__ import annotations
 
+import ctypes as C
 from collections import deque
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence
@@ -248,3 +249,88 @@ class RolloutRunner:
             res.ob_sum = sum(h.ob_sum for h in self.halves).cpu().numpy()
             res.ob_sumsq = sum(h.ob_sumsq for h in self.halves).cpu().numpy()
         return res
+
+
+class EpisodeKernelRunner:
+    """``RolloutRunner`` for environments whose episodes run entirely on the device (``env.device_episodes``; today
+    ``dne.envs.CartPoleEnv``): every member of every unit plays its whole episode inside ONE ``dne_cartpole_episodes``
+    launch, followed by one host sync for the results.  Same ``run`` signature and ``RolloutResult`` as ``RolloutRunner``.
+
+    Members are flattened in (unit, member) order; row ``u*G + g`` starts from row ``u*G + g`` of one
+    ``env.initial_states(n_units*G)`` call per ``run``."""
+
+    def __init__(self, ctx: F.Context, net: NetSpec, env: BatchEnv, n_slots: int = 0, group: int = 2, pipeline: int = 1,
+                 ref_batch: Optional[torch.Tensor] = None):
+        assert getattr(env, "device_episodes", False), "EpisodeKernelRunner needs an environment with device episodes"
+        if net.needs_ref_batch:
+            raise NotImplementedError("the episode kernel runs nets without batch norm only")
+        self.ctx, self.net, self.env, self.n_slots, self.G = ctx, net, env, n_slots, group
+        self.device = torch.device("cuda", ctx.device)
+        self.halves = (None,)          # one launch covers every member (drivers read len(halves) as tables per launch)
+        self.use_theta_idx = False
+        self.action_fn = None          # accepted for interface parity; the kernel's head is the argmax over 2 actions
+
+    def run(self, theta: torch.Tensor, units: List[Unit], timestep_limit: Optional[int] = None, *, ob_mean=None,
+            ob_std=None, collect_bc: Optional[str] = None, ac_noise_std: float = 0.0,
+            random_stream: Optional[np.random.RandomState] = None, save_obs_prob: float = 0.0) -> RolloutResult:
+        """Evaluate every unit once.  ``collect_bc``: None | 'final' (float64 [4] state after the last step)."""
+        if ob_mean is not None or ob_std is not None:
+            raise NotImplementedError("the episode kernel does not normalise observations")
+        if collect_bc not in (None, "final"):
+            raise NotImplementedError(f"collect_bc={collect_bc!r}: the episode kernel records the final state only")
+        if save_obs_prob != 0.0:
+            raise NotImplementedError("the episode kernel does not sample observation statistics")
+        if ac_noise_std != 0.0:
+            raise NotImplementedError("the episode kernel acts without action noise")
+        G, env = self.G, self.env
+        n_units = len(units)
+        n = n_units * G
+        limit = env.max_episode_steps if timestep_limit is None else min(timestep_limit, env.max_episode_steps)
+        assert limit is not None and limit >= 1
+        res = RolloutResult(np.zeros((n_units, G), np.float32), np.zeros((n_units, G), np.float32),
+                            np.zeros((n_units, G), np.int32), [[None] * G for _ in range(n_units)] if collect_bc else None)
+        self.use_theta_idx = theta.dim() == 2 and theta.shape[0] > 1
+        if n == 0:
+            return res
+        noise_idx = np.repeat(np.array([u.noise_idx for u in units], dtype=np.int64), G)
+        scale = np.array([u.scales[g] for u in units for g in range(G)], dtype=np.float32)
+        init = env.initial_states(n)
+        dev = self.device
+        d_idx = torch.from_numpy(noise_idx).to(dev)
+        d_scale = torch.from_numpy(scale).to(dev)
+        d_row = torch.from_numpy(np.repeat(np.array([u.theta_idx for u in units], dtype=np.int32), G)).to(dev) \
+            if self.use_theta_idx else None
+        d_init = torch.from_numpy(np.ascontiguousarray(init, dtype=np.float64)).to(dev)
+        d_ret = torch.empty(n, dtype=torch.float32, device=dev)
+        d_len = torch.empty(n, dtype=torch.int32, device=dev)
+        d_fin = torch.empty(n, 4, dtype=torch.float64, device=dev) if collect_bc == "final" else None
+        theta = theta.contiguous()
+        F.check(F.lib().dne_cartpole_episodes(
+            self.ctx.handle, C.byref(self.net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx),
+            F.ptr(d_scale), F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ret), F.ptr(d_len), F.ptr(d_fin),
+            F.stream_ptr()))
+        h_ret = torch.empty(n, dtype=torch.float32, pin_memory=True)
+        h_len = torch.empty(n, dtype=torch.int32, pin_memory=True)
+        h_ret.copy_(d_ret, non_blocking=True)
+        h_len.copy_(d_len, non_blocking=True)
+        if d_fin is not None:
+            h_fin = torch.empty(n, 4, dtype=torch.float64, pin_memory=True)
+            h_fin.copy_(d_fin, non_blocking=True)
+        torch.cuda.current_stream().synchronize()                 # the one host sync of the run
+        res.returns[:] = h_ret.numpy().reshape(n_units, G)
+        res.lengths[:] = h_len.numpy().reshape(n_units, G)
+        res.signreturns[:] = res.lengths                          # every reward is +1
+        res.steps = int(res.lengths.sum())
+        res.ticks = 1
+        if d_fin is not None:
+            fin = h_fin.numpy().reshape(n_units, G, 4)
+            res.bcs = [[fin[u, g].copy() for g in range(G)] for u in range(n_units)]
+        return res
+
+
+def make_runner(ctx: F.Context, net: NetSpec, env: BatchEnv, **kw):
+    """The rollout runner for ``env``: ``EpisodeKernelRunner`` when its episodes run on the device
+    (``env.device_episodes``), else the per-tick ``RolloutRunner``.  ``kw`` are ``RolloutRunner``'s arguments."""
+    if getattr(env, "device_episodes", False):
+        return EpisodeKernelRunner(ctx, net, env, **kw)
+    return RolloutRunner(ctx, net, env, **kw)

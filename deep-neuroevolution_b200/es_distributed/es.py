@@ -24,7 +24,7 @@ from dne import shard
 from dne.engine import ESUpdate, make_context
 from dne.envs import BatchEnv, make_env
 from dne.noise import SharedNoiseTable
-from dne.rollout import RolloutRunner, Unit
+from dne.rollout import Unit, make_runner
 
 logger = logging.getLogger(__name__)
 
@@ -346,7 +346,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     tslimit, incr_tslimit_threshold, tslimit_incr_ratio, tslimit_max, adaptive_tslimit = _cutoff(config)
     vine = bool(exp.get('vine_export'))        # es_modified.py: per-generation BC point clouds for the visual inspector
     group = 2
-    runner = RolloutRunner(ctx, policy.net, env, n_slots=n_slots, group=group,
+    runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=group,
                            pipeline=2 if n_slots % 4 == 0 else 1, ref_batch=policy.ref_batch)
     if getattr(policy, "_bin_values", None) is not None:
         runner.action_fn = policy.action_fn

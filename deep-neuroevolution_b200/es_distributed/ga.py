@@ -24,7 +24,7 @@ import torch
 
 from dne import _ffi as F
 from dne import shard
-from dne.rollout import RolloutRunner, Unit
+from dne.rollout import Unit, make_runner
 from .es import (Config, Result, Task, RunningStat, SharedNoiseTable, default_context, default_noise,   # noqa: F401
                  set_default_noise, setup as _es_setup, _cutoff, reference_row)
 
@@ -101,7 +101,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     elite = None
     deep_stats, deep_extra = {}, {}
     cache = GenomeCache(ctx, policy.net, config.noise_stdev, exp.get('ga_mode', 'cpu'))
-    runner = RolloutRunner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
+    runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
     population, population_score = [], np.array([], dtype=np.float32)
     episodes_so_far = timesteps_so_far = 0
     tstart = time.time()

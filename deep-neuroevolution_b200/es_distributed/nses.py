@@ -24,7 +24,7 @@ import torch
 
 from dne import _ffi as F
 from dne import shard
-from dne.rollout import RolloutRunner, Unit
+from dne.rollout import Unit, make_runner
 from .es import (Config, Result, Task, RunningStat, SharedNoiseTable, default_context, default_noise,   # noqa: F401
                  set_default_noise, setup as _es_setup, _cutoff, _process_returns, get_ref_batch, reference_row)
 
@@ -132,7 +132,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     tslimit, incr_thr, incr_ratio, tslimit_max, adaptive = _cutoff(config)
     if policy.needs_ref_batch:
         policy.set_ref_batch(get_ref_batch(env, batch_size=128, rs=np.random.RandomState(seed)))
-    runner = RolloutRunner(ctx, policy.net, env, n_slots=n_slots, group=2, pipeline=2 if n_slots % 4 == 0 else 1,
+    runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=2, pipeline=2 if n_slots % 4 == 0 else 1,
                            ref_batch=policy.ref_batch)
     if getattr(policy, "_bin_values", None) is not None:
         runner.action_fn = policy.action_fn

@@ -18,7 +18,7 @@ import torch
 from dne import _ffi as F
 from dne import nets as N
 from dne.engine import SlotForward
-from dne.rollout import RolloutRunner, Unit
+from dne.rollout import Unit, make_runner
 
 logger = logging.getLogger(__name__)
 
@@ -217,7 +217,7 @@ class Policy:
     def rollout(self, env, *, render=False, timestep_limit=None, save_obs=False, random_stream=None, **_):
         """policies.py:71-97 -- one episode of the CURRENT weights on slot 0 of a ``dne.envs.BatchEnv``.
         Returns (rews_sum_as_array, t, novelty_vector) like the Atari variants (policies.py:429,513)."""
-        runner = RolloutRunner(self._ctx, self.net, env, n_slots=2, group=1, pipeline=1, ref_batch=self.ref_batch)
+        runner = make_runner(self._ctx, self.net, env, n_slots=2, group=1, pipeline=1, ref_batch=self.ref_batch)
         res = runner.run(self._theta, [Unit(0, (0.0,))], timestep_limit, ob_mean=self.ob_mean, ob_std=self.ob_std,
                          collect_bc="final", ac_noise_std=getattr(self, "ac_noise_std", 0.0), random_stream=random_stream)
         return np.array([res.returns[0, 0]], dtype=np.float32), int(res.lengths[0, 0]), res.bcs[0][0]
@@ -314,6 +314,45 @@ class LargeModelPolicy(GAAtariPolicy):
 
     def _layer_names(self):
         return ["conv1", "conv2", "conv3", "fc", "out"]
+
+
+class SimpleClassifierPolicy(Policy):
+    """The reference GPU path's ``SimpleClassifier`` (gpu_implementation/neuroevolution/models/simple.py:29-34): fc1 16 relu,
+    fc2 16 relu, linear head over a ``Discrete`` action space, on ``Box`` vector observations (CartPole-v1: P = 386).
+    Normc init like ``GAAtariPolicy``; no observation normalisation."""
+    model_name = "SimpleClassifier"
+
+    def _initialize(self, ob_space, ac_space):
+        assert len(ob_space.shape) == 1, "vector (Box) observations"
+        assert hasattr(ac_space, "n"), "a Discrete action space"
+        self.ob_space_shape = ob_space.shape
+        self.ac_space = ac_space
+        self.num_actions = ac_space.n
+        return N.make_net(self.model_name, num_actions=self.num_actions, ob_dim=int(ob_space.shape[0]))
+
+    def _layer_names(self):
+        return ["fc1", "fc2", "out"]
+
+    def _initial_theta(self, rs):
+        theta = np.zeros(self.net.num_params, dtype=np.float32)
+        for l in self.net.layers:
+            theta[l.off_w:l.off_w + l.w_size] = _normc(rs, (l.cin, l.cout), l.std).reshape(-1)
+        return theta
+
+    @property
+    def needs_ob_stat(self):
+        return False
+
+    def act(self, ob, random_stream=None):
+        return np.argmax(self._forward_noiseless(np.asarray(ob, dtype=np.float32)), axis=1).astype(np.int64)
+
+
+class LinearClassifierPolicy(SimpleClassifierPolicy):
+    """The reference GPU path's ``LinearClassifier`` (simple.py:23-27): one linear layer 'out' (CartPole-v1: P = 10)."""
+    model_name = "LinearClassifier"
+
+    def _layer_names(self):
+        return ["out"]
 
 
 class MujocoPolicy(Policy):

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from dne import shard
-from dne.rollout import RolloutRunner, Unit
+from dne.rollout import Unit, make_runner
 from .es import SharedNoiseTable, default_context, default_noise, set_default_noise, _cutoff, reference_row   # noqa: F401
 from .ga import GenomeCache, setup
 
@@ -43,7 +43,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     dev = policy.device
     tslimit, incr_thr, incr_ratio, _, adaptive = _cutoff(config)
     cache = GenomeCache(ctx, policy.net, config.noise_stdev, exp.get('ga_mode', 'cpu'))
-    runner = RolloutRunner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
+    runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
     chunk = torch.empty(n_slots, P, dtype=torch.float32, device=dev)
     best_score, best_seed = float('-inf'), None                   # rs.py:35
     episodes_so_far = timesteps_so_far = 0

@@ -166,6 +166,19 @@ int dne_perturb_forward_mlp(dne_ctx* ctx, const dne_net_desc* net, const float* 
                             const float* d_obs, const float* d_ob_mean, const float* d_ob_std,
                             float* d_actions_out, void* d_ws, size_t ws_bytes, void* stream);
 
+/* CartPole-v1 (gym classic_control) episodes run entirely on the device, one per member:
+ * weights theta[d_theta_idx[m] or 0] + d_scale[m]*noise[d_noise_idx[m] : +P], initial state d_init_state[m][4] (float64),
+ * at most max_steps steps.  Outputs d_returns float[n], d_lengths int32[n], d_final_state double[n][4] (nullable:
+ * state after the last step -- the 'final' behaviour characterisation).  Enqueued on `stream`, no host sync.
+ * Supported nets (SimpleClassifier / LinearClassifier shapes): 1..4 dense layers of width <= 32, DNE_OB_VECTOR with
+ * ob_dim 4, n_out 2, ReLU hidden layers, linear head, no batch norm; anything else returns DNE_ERR_UNSUP.
+ * Observation = (float)state; action = argmax of the logits (first max on ties, NaN counts as the maximum); the
+ * environment step is float64 in gym's operation order; return = length (reward 1 per step). */
+int dne_cartpole_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                          const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                          int n_members, const double* d_init_state, int max_steps,
+                          float* d_returns, int32_t* d_lengths, double* d_final_state, void* stream);
+
 /* Observation statistics of the running normaliser (es.py:356-363 rollout_and_update_ob_stat; RunningStat es.py:26-48):
  * adds the observations d_obs[slot, :] (float32 [*, ob_dim], the unnormalised vectors fed to this tick's forward) of the m
  * listed slots -- the slots whose episode was sampled with probability calc_obstat_prob -- into float64 running sums

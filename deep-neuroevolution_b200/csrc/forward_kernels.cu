@@ -384,14 +384,16 @@ dense_combine_kernel(SlotArgs sa, LayerEpi epi, int n_slots, int N, int G, const
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Small / irregular dense layer (output heads: 512x18, 256x17; anything with N % 4 != 0), one CTA per slot,
-// fused w = theta + s*noise, optional argmax (policies.py:330: first max on ties, NaN counts as max).
+// Small / irregular dense layer (output heads: 512x18, 256x17; anything with N % 4 != 0), one CTA per slot and tile
+// of up to DS_MAXN output columns, fused w = theta + s*noise, optional argmax (policies.py:330: first max on ties, NaN
+// counts as max; only for N <= DS_MAXN, a single tile).
 // ---------------------------------------------------------------------------------------------------
 constexpr int DS_THREADS = 256, DS_MAXN = 256;
 
-// Thread t < RG*N owns output column n = t % N and row group rg = t / N (RG = 256 / N row groups): one iteration
-// of the k loop covers RG consecutive rows = RG*N CONTIGUOUS weights, so the theta / noise loads are flat and
-// perfectly coalesced whatever N is (18, 17, ...).
+// Column tile blockIdx.y covers columns [n0, n0 + NT).  Thread t < RG*NT owns output column n0 + t % NT and row group
+// rg = t / NT (RG = 256 / NT row groups).  With a single tile (N <= 256), one iteration of the k loop covers RG
+// consecutive rows = RG*N CONTIGUOUS weights, so the theta / noise loads are flat and perfectly coalesced whatever N
+// is (18, 17, ...); wider layers read NT contiguous weights per row.
 __global__ void __launch_bounds__(DS_THREADS)
 dense_small_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const float* __restrict__ X, int64_t x_slot_stride,
                    int K, int N, float* __restrict__ out, int64_t out_slot_stride, int32_t* __restrict__ actions) {
@@ -399,14 +401,16 @@ dense_small_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const float* __rest
     if (!slot_active(sa, slot)) return;
     __shared__ float red[DS_THREADS];
     __shared__ float ys[DS_MAXN];
-    const int RG = DS_THREADS / N;
+    const int n0 = blockIdx.y * DS_MAXN;
+    const int NT = min(DS_MAXN, N - n0);
+    const int RG = DS_THREADS / NT;
     const int t = threadIdx.x;
-    const int n = t % N, rg = t / N;
+    const int n = t % NT, rg = t / NT;
     const float* th = slot_theta(sa, slot);
     const int64_t idx = sa.noise_idx[slot];
     const float s = sa.scale[slot];
-    const float* tw = th + off_w;
-    const float* nz = sa.noise + idx + off_w;
+    const float* tw = th + off_w + n0;
+    const float* nz = sa.noise + idx + off_w + n0;
     const float* x = X + (int64_t)slot * x_slot_stride;
     float acc0 = 0.0f, acc1 = 0.0f;
     if (rg < RG) {
@@ -424,16 +428,16 @@ dense_small_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const float* __rest
     }
     red[t] = acc0 + acc1;
     __syncthreads();
-    if (t < N) {
+    if (t < NT) {
         float sum = 0.0f;
-        for (int g = 0; g < RG; ++g) sum += red[g * N + t];
-        const ChanEpi ce = make_chan_epi(sa, epi, slot, N, t, th, idx, s);
+        for (int g = 0; g < RG; ++g) sum += red[g * NT + t];
+        const ChanEpi ce = make_chan_epi(sa, epi, slot, N, n0 + t, th, idx, s);
         const float y = ce.apply(sum);
         ys[t] = y;
-        if (out) out[(int64_t)slot * out_slot_stride + t] = y;
+        if (out) out[(int64_t)slot * out_slot_stride + n0 + t] = y;
     }
     __syncthreads();
-    if (actions && threadIdx.x == 0) {
+    if (actions && threadIdx.x == 0) {             // N <= DS_MAXN (dne_launch_dense_layer): one tile holds every column
         int best = 0;
         float bv = ys[0];
         for (int j = 1; j < N; ++j) {
@@ -567,15 +571,16 @@ dense_combine_head_kernel(SlotArgs sa, LayerEpi epi1, int n_slots, int N1, int G
     }
 }
 
-// MujocoPolicy observation normalisation (policies.py:151): clip((o - mean) / std, -5, 5)
+// MujocoPolicy observation normalisation (policies.py:151): clip((o - mean) / std, -5, 5).  Without statistics (mean
+// NULL: SimpleClassifier / LinearClassifier, models/simple.py) the observation goes through unchanged and unclipped.
 __global__ void ob_norm_kernel(const float* __restrict__ obs, const float* __restrict__ mean,
                                const float* __restrict__ stdv, int64_t total, int dim, float* __restrict__ out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const int d = (int)(i % dim);
     float v = obs[i];
-    if (mean) v = __fdiv_rn(__fsub_rn(v, mean[d]), stdv[d]);
-    out[i] = fminf(fmaxf(v, -5.0f), 5.0f);
+    if (mean) v = fminf(fmaxf(__fdiv_rn(__fsub_rn(v, mean[d]), stdv[d]), -5.0f), 5.0f);
+    out[i] = v;
 }
 
 // Observation statistics for the running normaliser (es.py:356-363: task_ob_stat.increment(obs.sum(0), square(obs).sum(0),
@@ -706,9 +711,9 @@ int dne_launch_dense_layer(const dne_ctx* ctx, const SlotArgs& sa, const dne_lay
                            int n_slots, cudaStream_t st, const DenseHead* head, const TgmOperands* tgm) {
     const int K = L.cin, N = L.cout;
     if (!p.decomposed) {
-        if (N > DS_MAXN) return DNE_ERR_UNSUP;
-        dense_small_kernel<<<n_slots, DS_THREADS, 0, st>>>(sa, L.off_w, epi, X, x_slot_stride, K, N, out,
-                                                          out_slot_stride, actions);
+        if (actions && N > DS_MAXN) return DNE_ERR_UNSUP;          // the argmax runs over one column tile
+        dense_small_kernel<<<dim3(n_slots, (N + DS_MAXN - 1) / DS_MAXN), DS_THREADS, 0, st>>>(
+            sa, L.off_w, epi, X, x_slot_stride, K, N, out, out_slot_stride, actions);
         DNE_LAUNCHED(1);
         return 0;
     }

@@ -102,6 +102,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     deep_stats, deep_extra = {}, {}
     cache = GenomeCache(ctx, policy.net, config.noise_stdev, exp.get('ga_mode', 'cpu'))
     runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
+    ob_stat = dict(ob_mean=policy.ob_mean, ob_std=policy.ob_std)            # MujocoPolicy: its fixed statistics
     population, population_score = [], np.array([], dtype=np.float32)
     episodes_so_far = timesteps_so_far = 0
     tstart = time.time()
@@ -126,7 +127,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
             l_loc = np.zeros(hi - lo, np.int32)
             if len(population) > 0:
                 units = [Unit(new_seeds[i], (np.float32(config.noise_stdev),), parents[i]) for i in range(lo, hi)]
-                res = runner.run(cache.theta, units, tslimit)
+                res = runner.run(cache.theta, units, tslimit, **ob_stat)
                 r_loc[:], l_loc[:] = res.returns[:, 0], res.lengths[:, 0]
             else:
                 # generation 0: theta = reinitialize(noise[seed]) per offspring, a slot-table full at a time
@@ -136,7 +137,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
                     for j in range(c0, c1):
                         cache.materialize(batch[j], chunk[j - c0])
                     units = [Unit(0, (0.0,), j - c0) for j in range(c0, c1)]
-                    res = runner.run(chunk, units, tslimit)
+                    res = runner.run(chunk, units, tslimit, **ob_stat)
                     r_loc[c0 - lo:c1 - lo], l_loc[c0 - lo:c1 - lo] = res.returns[:, 0], res.lengths[:, 0]
             pack = torch.from_numpy(np.stack([r_loc, l_loc.astype(np.float32)], axis=1)).to(dev)
             allr = shard.all_gather_rows(pack, n_off).cpu().numpy()
@@ -176,7 +177,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
                     cache.materialize(gnm, val_theta[j])
             v_units = [Unit(0, (0.0,), j) for j in range(len(val_pop)) for _ in range(n_val)]
             vlo, vhi = shard.shard_bounds(len(v_units), rank, world)
-            vres = runner.run(val_theta, v_units[vlo:vhi], tslimit)
+            vres = runner.run(val_theta, v_units[vlo:vhi], tslimit, **ob_stat)
             vpack = torch.from_numpy(np.stack([vres.returns[:, 0], vres.lengths[:, 0].astype(np.float32)], axis=1)).to(dev)
             vall = shard.all_gather_rows(vpack, len(v_units)).cpu().numpy()
             val_returns = vall[:, 0].reshape(len(val_pop), n_val)

@@ -358,6 +358,13 @@ class LinearClassifierPolicy(SimpleClassifierPolicy):
 class MujocoPolicy(Policy):
     """policies.py:122-302 ('ff' connection; 'continuous:', 'uniform:N' and 'custom:v0,..,vk' action heads)."""
 
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        # Observation statistics from the start: mean 0 / std 1 (the master's initial RunningStat, es.py:26-48) keeps
+        # the clip to [-5, 5] on every forward; the engine does not clip inputs fed without statistics.
+        dim = int(self.net.ob_dim)
+        self.set_ob_stat(np.zeros(dim, np.float32), np.ones(dim, np.float32))
+
     def _initialize(self, ob_space, ac_space, ac_bins, ac_noise_std, nonlin_type, hidden_dims, connection_type):
         self.ac_space = ac_space
         self.ac_bins = ac_bins

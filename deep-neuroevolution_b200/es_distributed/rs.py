@@ -44,6 +44,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     tslimit, incr_thr, incr_ratio, _, adaptive = _cutoff(config)
     cache = GenomeCache(ctx, policy.net, config.noise_stdev, exp.get('ga_mode', 'cpu'))
     runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
+    ob_stat = dict(ob_mean=policy.ob_mean, ob_std=policy.ob_std)            # MujocoPolicy: its fixed statistics
     chunk = torch.empty(n_slots, P, dtype=torch.float32, device=dev)
     best_score, best_seed = float('-inf'), None                   # rs.py:35
     episodes_so_far = timesteps_so_far = 0
@@ -68,7 +69,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
                 for j in range(c0, c1):
                     cache.materialize((batch[j],), chunk[j - c0])          # theta = reinitialize(noise[seed])
                 units = [Unit(0, (0.0,), j - c0) for j in range(c0, c1)]
-                res = runner.run(chunk, units, tslimit)
+                res = runner.run(chunk, units, tslimit, **ob_stat)
                 r_loc[c0 - lo:c1 - lo], l_loc[c0 - lo:c1 - lo] = res.returns[:, 0], res.lengths[:, 0]
             pack = torch.from_numpy(np.stack([r_loc, l_loc.astype(np.float32)], axis=1)).to(dev)
             allr = shard.all_gather_rows(pack, n_cand).cpu().numpy()

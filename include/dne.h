@@ -50,7 +50,8 @@ extern "C" {
 
 /* observation kinds */
 #define DNE_OB_ATARI_U8 0      /* uint8 [slots,84,84,4], scaled by 1/255 (atari_wrappers.py:186) */
-#define DNE_OB_VECTOR   1      /* float32 [slots,ob_dim], clip((o-mean)/std,-5,5) (policies.py:151) */
+#define DNE_OB_VECTOR   1      /* float32 [slots,ob_dim], clip((o-mean)/std,-5,5) (policies.py:151); without
+                                  statistics (d_ob_mean NULL) used as given, unclipped */
 
 typedef struct dne_layer_desc {
     int32_t kind;              /* DNE_CONV | DNE_DENSE */
@@ -159,7 +160,11 @@ int dne_theta_forget(dne_ctx* ctx, const void* d_ws);
 int dne_set_phase_events(dne_ctx* ctx, void* wait_event, void* record_event, int mode);
 
 /* MujocoPolicy variant (policies.py:150-162,195-196,202-206): float observations, ob normalisation, tanh MLP,
- * continuous head.  d_actions_out float[n_slots, n_out] (action noise is added by the caller's stream). */
+ * continuous head.  d_actions_out float[n_slots, n_out] (action noise is added by the caller's stream).
+ * d_ob_mean / d_ob_std (both or neither): the layer input is clip((o - mean) / std, -5, 5).  Both NULL: the
+ * observations are fed as they are, NOT clipped (SimpleClassifier / LinearClassifier, models/simple.py: no
+ * normalisation).  A MujocoPolicy always passes statistics (mean 0 / std 1 before its first set_ob_stat).
+ * Dense layers of any width run; an output wider than 256 has no argmax (dne_perturb_forward_conv: DNE_ERR_UNSUP). */
 int dne_perturb_forward_mlp(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
                             const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
                             const uint8_t* d_active, int n_slots, int paired,

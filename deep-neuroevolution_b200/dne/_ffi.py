@@ -52,6 +52,9 @@ _SIGS = {
                                 C.c_size_t, _P],
     "dne_ob_stat_accumulate": [_P, C.c_int, _P, C.c_int, _P, _P, _P],
     "dne_cartpole_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P],
+    "dne_pendulum_net_supported": [C.POINTER(NetDesc)],
+    "dne_pendulum_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
+                              _P, _P, _P],
     "dne_theta_prepare": [_P, C.POINTER(NetDesc), _P, C.c_int, _P, C.c_size_t, _P],
     "dne_theta_forget": [_P, _P],
     "dne_vbn_ws_bytes": [C.POINTER(NetDesc), C.c_int, C.c_int, C.POINTER(C.c_size_t)],

@@ -9,15 +9,24 @@ Step`` over a batch of ALE instances (gpu_implementation/gym_tensorflow/tf_env.c
 ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so the environment shipped
 here is the synthetic Frostbite-shaped stub the measurement plan names (SURVEY.md 8d): i.i.d. uint8 84x84x4
 observations from a fixed pool, rewards 10*Bernoulli(0.05), fixed or ragged episode lengths.  A real emulator
-plugs in by subclassing ``BatchEnv``.  One real task needs no emulator: CartPole-v1 (``CartPoleEnv``), whose episodes run
-whole on the device (``dne.rollout.EpisodeKernelRunner``).
+plugs in by subclassing ``BatchEnv``.  Two real tasks need no emulator: CartPole-v1 (``CartPoleEnv``) and Pendulum-v1
+(``PendulumEnv``), whose episodes run whole on the device (``dne.rollout.EpisodeKernelRunner``).
+
+An environment with device episodes (``device_episodes = True``) supplies ``state_dim``, ``initial_states(k)``,
+``episode_net_supported(net)`` and ``launch_episodes(...)``; ``kernel_policy_io`` says whether its kernel also takes
+observation statistics, action noise and observation sums (MujocoPolicy), and ``host_step`` whether the per-tick
+``RolloutRunner`` can step it on the host instead.
 """
 from __future__ import annotations
 
 from typing import Optional, Sequence
 
+import ctypes as C
+
 import numpy as np
 import torch
+
+from . import _ffi as F
 
 
 class Discrete:
@@ -201,8 +210,8 @@ class SyntheticVectorEnv(BatchEnv):
 def make_env(env_id: str, n_slots: int, seed: int = 0, episode_len=None, allow_synthetic: bool = False, **kw) -> BatchEnv:
     """``gym.make(exp['env_id'])`` (es.py:131) for a whole slot table.
 
-    ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so apart from CartPole-v1
-    (``CartPoleEnv``, registered in ``ENV_BACKENDS``) the only backends here are the synthetic stubs.  They are returned for the explicit ids ``SyntheticAtari*`` / ``SyntheticVector*``; for a REAL id
+    ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so apart from CartPole-v1 and
+    Pendulum-v1 (``CartPoleEnv``, ``PendulumEnv``, registered in ``ENV_BACKENDS``) the only backends here are the synthetic stubs.  They are returned for the explicit ids ``SyntheticAtari*`` / ``SyntheticVector*``; for a REAL id
     (``FrostbiteNoFrameskip-v4``, ``Humanoid-v1`` ...) they are returned only when the caller opts in
     (``exp['allow_synthetic_env'] = true`` or ``DNE_ALLOW_SYNTHETIC_ENV=1``), with a loud warning -- a run that silently
     optimised random frames while logging and snapshotting like a real one would be worse than an error.  A real emulator
@@ -235,9 +244,12 @@ def make_env(env_id: str, n_slots: int, seed: int = 0, episode_len=None, allow_s
 class CartPoleEnv(BatchEnv):
     """gym's CartPole-v1 (classic_control cartpole.py) for a whole population, stepped ON THE DEVICE: whole episodes run in
     one launch of ``dne_cartpole_episodes`` (``dne.rollout.EpisodeKernelRunner``), so this object only supplies the spaces,
-    the time limit and the reset states.  ``initial_states(k)`` draws k resets ``uniform(-0.05, 0.05, size=4)`` from one
-    ``RandomState(seed)`` stream that continues across calls, as one gym env reset k times in a row would."""
+    the time limit, the reset states and the launch.  ``initial_states(k)`` draws k resets ``uniform(-0.05, 0.05, size=4)``
+    from one ``RandomState(seed)`` stream that continues across calls, as one gym env reset k times in a row would."""
     device_episodes = True
+    host_step = False
+    kernel_policy_io = False       # no observation normalisation, action noise or observation statistics in the kernel
+    state_dim = 4
 
     def __init__(self, n_slots: int, seed: int = 0):
         self.n_slots = int(n_slots)
@@ -252,6 +264,16 @@ class CartPoleEnv(BatchEnv):
         """float64 [k, 4] reset states (gym ``reset``: ``uniform(low=-0.05, high=0.05, size=(4,))`` per episode)."""
         return self.rs.uniform(-0.05, 0.05, size=(int(k), 4))
 
+    def episode_net_supported(self, net) -> bool:
+        return True                # the only path: dne_cartpole_episodes itself rejects a net it cannot run
+
+    def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
+                        **_):
+        F.check(F.lib().dne_cartpole_episodes(
+            ctx.handle, C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale), F.ptr(d_row), n,
+            F.ptr(d_init), int(limit), F.ptr(d_ret), F.ptr(d_len), F.ptr(d_fin), F.stream_ptr()))
+        d_sret.copy_(d_ret)        # every reward is +1: the sign-return is the return
+
     def _host_stepping(self, *a, **kw):
         raise NotImplementedError("CartPoleEnv runs whole episodes on the device: use dne.rollout.make_runner "
                                   "(EpisodeKernelRunner), not the per-tick host reset / step")
@@ -264,7 +286,82 @@ def _make_cartpole(env_id, n_slots, seed=0, episode_len=None, **kw):
     return CartPoleEnv(n_slots, seed=seed)
 
 
+class PendulumEnv(BatchEnv):
+    """gymnasium's Pendulum-v1 (classic_control pendulum.py; DESIGN.md 3.6) for a whole population.  Whole episodes run on the
+    device in one launch of ``dne_pendulum_episodes`` (``dne.rollout.EpisodeKernelRunner``); for nets that kernel does not
+    take (wider hidden layers, discretised heads whose ``action_fn`` runs on the host) the same dynamics step here, on the
+    host, vectorised in numpy float64 in the same operation order, under the per-tick ``RolloutRunner``.  There is no
+    termination; TimeLimit 200.  Resets draw ``uniform(low=[-pi, -1], high=[pi, 1])`` per episode from one
+    ``RandomState(seed)`` stream that continues across calls (``initial_states`` and ``reset`` share it).  ``get_ram``
+    returns the state ``(th, thdot)``: the 'final' behaviour characterisation."""
+    device_episodes = True
+    host_step = True
+    kernel_policy_io = True
+    state_dim = 2
+    HIGH = np.array([np.pi, 1.0])
+
+    def __init__(self, n_slots: int, seed: int = 0, pin: bool = True):
+        self.n_slots = int(n_slots)
+        self.observation_space = Box(np.array([-1.0, -1.0, -8.0], np.float32), np.array([1.0, 1.0, 8.0], np.float32))
+        self.action_space = Box(-2.0, 2.0, (1,))
+        self.max_episode_steps = 200                                             # TimeLimit of Pendulum-v1
+        self.rs = np.random.RandomState(seed)
+        self.state = np.zeros((self.n_slots, 2), dtype=np.float64)
+        obs = torch.zeros(self.n_slots, 3, dtype=torch.float32)
+        self.obs = obs.pin_memory() if (pin and torch.cuda.is_available()) else obs
+
+    def initial_states(self, k: int) -> np.ndarray:
+        """float64 [k, 2] reset states (th, thdot)."""
+        return self.rs.uniform(low=-self.HIGH, high=self.HIGH, size=(int(k), 2))
+
+    def episode_net_supported(self, net) -> bool:
+        return F.lib().dne_pendulum_net_supported(C.byref(net.desc)) == 0
+
+    def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
+                        d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None):
+        F.check(F.lib().dne_pendulum_episodes(
+            ctx.handle, C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale), F.ptr(d_row), n,
+            F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise), F.ptr(d_ret), F.ptr(d_sret),
+            F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq), F.stream_ptr()))
+
+    def _write_obs(self, slots):
+        th, thdot = self.state[slots, 0], self.state[slots, 1]
+        self.obs[torch.from_numpy(slots)] = torch.from_numpy(np.stack([np.cos(th), np.sin(th), thdot], axis=1)
+                                                             .astype(np.float32))
+
+    def reset(self, slots):
+        slots = np.asarray(slots, dtype=np.int64)
+        self.state[slots] = self.initial_states(len(slots))
+        self._write_obs(slots)
+
+    def step(self, slots, actions):
+        """gymnasium ``step`` for the listed slots; ``actions`` float32 [k, 1].  Rewards float32 [k], done all False."""
+        slots = np.asarray(slots, dtype=np.int64)
+        u = np.clip(np.asarray(actions, dtype=np.float32).reshape(len(slots), 1), -2.0, 2.0)[:, 0]   # float32
+        th, thdot = self.state[slots, 0], self.state[slots, 1]
+        an = np.mod(th + np.pi, 2 * np.pi) - np.pi                                                    # angle_normalize
+        costs = an ** 2 + 0.1 * thdot ** 2 + 0.001 * (u * u).astype(np.float64)
+        newthdot = np.clip(thdot + (15.0 * np.sin(th) + 3.0 * u.astype(np.float64)) * 0.05, -8.0, 8.0)
+        self.state[slots, 0] = th + newthdot * 0.05
+        self.state[slots, 1] = newthdot
+        self._write_obs(slots)
+        return (-costs).astype(np.float32), np.zeros(len(slots), dtype=bool)
+
+    def get_ram(self, slots):
+        return self.state[np.asarray(slots, dtype=np.int64)].copy()
+
+    def random_actions(self, k, rs):
+        return rs.uniform(-2.0, 2.0, size=(k, 1)).astype(np.float32)
+
+
+def _make_pendulum(env_id, n_slots, seed=0, episode_len=None, **kw):
+    if episode_len is not None:
+        raise ValueError("Pendulum-v1 has a fixed 200-step time limit; use the episode cutoff of the config instead")
+    return PendulumEnv(n_slots, seed=seed, **kw)
+
+
 ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_len=, **kw) -> BatchEnv (real emulators plug in here)
     "CartPole-v1": _make_cartpole,
     "gym.CartPole-v1": _make_cartpole,   # the id of the reference GPU path's configurations/es_gym_config.json
+    "Pendulum-v1": _make_pendulum,
 }

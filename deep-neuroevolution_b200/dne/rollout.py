@@ -252,12 +252,16 @@ class RolloutRunner:
 
 
 class EpisodeKernelRunner:
-    """``RolloutRunner`` for environments whose episodes run entirely on the device (``env.device_episodes``; today
-    ``dne.envs.CartPoleEnv``): every member of every unit plays its whole episode inside ONE ``dne_cartpole_episodes``
-    launch, followed by one host sync for the results.  Same ``run`` signature and ``RolloutResult`` as ``RolloutRunner``.
+    """``RolloutRunner`` for environments whose episodes run entirely on the device (``env.device_episodes``:
+    ``dne.envs.CartPoleEnv``, ``dne.envs.PendulumEnv``): every member of every unit plays its whole episode inside ONE
+    launch (``env.launch_episodes``), followed by one host sync for the results.  Same ``run`` signature and
+    ``RolloutResult`` as ``RolloutRunner``.
 
     Members are flattened in (unit, member) order; row ``u*G + g`` starts from row ``u*G + g`` of one
-    ``env.initial_states(n_units*G)`` call per ``run``."""
+    ``env.initial_states(n_units*G)`` call per ``run``.  When the environment's kernel takes MujocoPolicy's inputs
+    (``env.kernel_policy_io``), ``run`` also draws, from ``random_stream``: first one ``rand()`` per non-noiseless member in
+    (unit, member) order against ``save_obs_prob`` (the members whose observations go into the statistics), then one
+    ``randn(n_noisy, limit, 1)`` of action noise for the non-noiseless members, scaled as ``RolloutRunner`` scales it."""
 
     def __init__(self, ctx: F.Context, net: NetSpec, env: BatchEnv, n_slots: int = 0, group: int = 2, pipeline: int = 1,
                  ref_batch: Optional[torch.Tensor] = None):
@@ -268,21 +272,23 @@ class EpisodeKernelRunner:
         self.device = torch.device("cuda", ctx.device)
         self.halves = (None,)          # one launch covers every member (drivers read len(halves) as tables per launch)
         self.use_theta_idx = False
-        self.action_fn = None          # accepted for interface parity; the kernel's head is the argmax over 2 actions
+        self.action_fn = None          # accepted for interface parity; the kernel's head is the environment's action
 
     def run(self, theta: torch.Tensor, units: List[Unit], timestep_limit: Optional[int] = None, *, ob_mean=None,
             ob_std=None, collect_bc: Optional[str] = None, ac_noise_std: float = 0.0,
             random_stream: Optional[np.random.RandomState] = None, save_obs_prob: float = 0.0) -> RolloutResult:
-        """Evaluate every unit once.  ``collect_bc``: None | 'final' (float64 [4] state after the last step)."""
-        if ob_mean is not None or ob_std is not None:
-            raise NotImplementedError("the episode kernel does not normalise observations")
+        """Evaluate every unit once.  ``collect_bc``: None | 'final' (float64 [env.state_dim] state after the last step)."""
+        G, env = self.G, self.env
+        if not env.kernel_policy_io:
+            if ob_mean is not None or ob_std is not None:
+                raise NotImplementedError("the episode kernel does not normalise observations")
         if collect_bc not in (None, "final"):
             raise NotImplementedError(f"collect_bc={collect_bc!r}: the episode kernel records the final state only")
-        if save_obs_prob != 0.0:
-            raise NotImplementedError("the episode kernel does not sample observation statistics")
-        if ac_noise_std != 0.0:
-            raise NotImplementedError("the episode kernel acts without action noise")
-        G, env = self.G, self.env
+        if not env.kernel_policy_io:
+            if save_obs_prob != 0.0:
+                raise NotImplementedError("the episode kernel does not sample observation statistics")
+            if ac_noise_std != 0.0:
+                raise NotImplementedError("the episode kernel acts without action noise")
         n_units = len(units)
         n = n_units * G
         limit = env.max_episode_steps if timestep_limit is None else min(timestep_limit, env.max_episode_steps)
@@ -290,47 +296,81 @@ class EpisodeKernelRunner:
         res = RolloutResult(np.zeros((n_units, G), np.float32), np.zeros((n_units, G), np.float32),
                             np.zeros((n_units, G), np.int32), [[None] * G for _ in range(n_units)] if collect_bc else None)
         self.use_theta_idx = theta.dim() == 2 and theta.shape[0] > 1
+        want_obstat = save_obs_prob != 0.0 and self.net.ob_kind == F.OB_VECTOR
+        if want_obstat:
+            res.ob_sum = np.zeros(self.net.ob_dim)
+            res.ob_sumsq = np.zeros(self.net.ob_dim)
         if n == 0:
             return res
         noise_idx = np.repeat(np.array([u.noise_idx for u in units], dtype=np.int64), G)
         scale = np.array([u.scales[g] for u in units for g in range(G)], dtype=np.float32)
         init = env.initial_states(n)
         dev = self.device
+        extra = {}
+        if env.kernel_policy_io:
+            noisy = ~np.repeat(np.array([u.noiseless for u in units], dtype=bool), G)
+            if want_obstat:                   # es.py:356-357, drawn in RolloutRunner's order (before any action noise)
+                stream = random_stream if random_stream is not None else np.random.RandomState(0)
+                save = np.zeros(n, dtype=bool)
+                save[noisy] = stream.rand(int(noisy.sum())) < save_obs_prob     # = one rand() per member, in order
+                extra["d_ob_sum"] = torch.empty(n, self.net.ob_dim, dtype=torch.float64, device=dev)
+                extra["d_ob_sumsq"] = torch.empty_like(extra["d_ob_sum"])
+            if ac_noise_std != 0.0 and random_stream is not None:          # policies.py:204-205, RolloutRunner.finish
+                ac = np.zeros((n, int(limit), self.net.n_out), dtype=np.float32)
+                ac[noisy] = random_stream.randn(int(noisy.sum()), int(limit), self.net.n_out).astype(np.float32) * \
+                    np.float32(ac_noise_std)
+                extra["d_ac_noise"] = torch.from_numpy(ac).to(dev)
+            if ob_mean is not None:
+                extra["d_ob_mean"] = ob_mean.to(dev, torch.float32).contiguous()
+                extra["d_ob_std"] = ob_std.to(dev, torch.float32).contiguous()
         d_idx = torch.from_numpy(noise_idx).to(dev)
         d_scale = torch.from_numpy(scale).to(dev)
         d_row = torch.from_numpy(np.repeat(np.array([u.theta_idx for u in units], dtype=np.int32), G)).to(dev) \
             if self.use_theta_idx else None
+        sd = env.state_dim
         d_init = torch.from_numpy(np.ascontiguousarray(init, dtype=np.float64)).to(dev)
         d_ret = torch.empty(n, dtype=torch.float32, device=dev)
+        d_sret = torch.empty(n, dtype=torch.float32, device=dev)
         d_len = torch.empty(n, dtype=torch.int32, device=dev)
-        d_fin = torch.empty(n, 4, dtype=torch.float64, device=dev) if collect_bc == "final" else None
+        d_fin = torch.empty(n, sd, dtype=torch.float64, device=dev) if collect_bc == "final" else None
         theta = theta.contiguous()
-        F.check(F.lib().dne_cartpole_episodes(
-            self.ctx.handle, C.byref(self.net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx),
-            F.ptr(d_scale), F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ret), F.ptr(d_len), F.ptr(d_fin),
-            F.stream_ptr()))
-        h_ret = torch.empty(n, dtype=torch.float32, pin_memory=True)
-        h_len = torch.empty(n, dtype=torch.int32, pin_memory=True)
-        h_ret.copy_(d_ret, non_blocking=True)
-        h_len.copy_(d_len, non_blocking=True)
-        if d_fin is not None:
-            h_fin = torch.empty(n, 4, dtype=torch.float64, pin_memory=True)
-            h_fin.copy_(d_fin, non_blocking=True)
+        env.launch_episodes(self.ctx, self.net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len,
+                            d_fin, **extra)
+        outs = {"ret": d_ret, "sret": d_sret, "len": d_len, "fin": d_fin,
+                "ob_sum": extra.get("d_ob_sum"), "ob_sumsq": extra.get("d_ob_sumsq")}
+        host = {}
+        for k, d in outs.items():
+            if d is not None:
+                host[k] = torch.empty(d.shape, dtype=d.dtype, pin_memory=True)
+                host[k].copy_(d, non_blocking=True)
         torch.cuda.current_stream().synchronize()                 # the one host sync of the run
-        res.returns[:] = h_ret.numpy().reshape(n_units, G)
-        res.lengths[:] = h_len.numpy().reshape(n_units, G)
-        res.signreturns[:] = res.lengths                          # every reward is +1
+        res.returns[:] = host["ret"].numpy().reshape(n_units, G)
+        res.signreturns[:] = host["sret"].numpy().reshape(n_units, G)
+        res.lengths[:] = host["len"].numpy().reshape(n_units, G)
         res.steps = int(res.lengths.sum())
         res.ticks = 1
         if d_fin is not None:
-            fin = h_fin.numpy().reshape(n_units, G, 4)
+            fin = host["fin"].numpy().reshape(n_units, G, sd)
             res.bcs = [[fin[u, g].copy() for g in range(G)] for u in range(n_units)]
+        if want_obstat:                       # the flagged members' sums, added in member order
+            s_, q_ = host["ob_sum"].numpy(), host["ob_sumsq"].numpy()
+            for m in np.nonzero(save)[0]:
+                res.ob_sum += s_[m]
+                res.ob_sumsq += q_[m]
+            res.ob_count = int(res.lengths.ravel()[save].sum())
         return res
 
 
-def make_runner(ctx: F.Context, net: NetSpec, env: BatchEnv, **kw):
+def make_runner(ctx: F.Context, net: NetSpec, env: BatchEnv, action_fn=None, **kw):
     """The rollout runner for ``env``: ``EpisodeKernelRunner`` when its episodes run on the device
-    (``env.device_episodes``), else the per-tick ``RolloutRunner``.  ``kw`` are ``RolloutRunner``'s arguments."""
-    if getattr(env, "device_episodes", False):
-        return EpisodeKernelRunner(ctx, net, env, **kw)
-    return RolloutRunner(ctx, net, env, **kw)
+    (``env.device_episodes``), the environment's kernel takes ``net`` (``env.episode_net_supported``) and no host
+    ``action_fn`` maps the network's output to actions; otherwise the per-tick ``RolloutRunner`` when the environment
+    has a host step.  ``action_fn``: the policy's map from output rows to actions (discretised MuJoCo heads), None for
+    the identity.  ``kw`` are ``RolloutRunner``'s arguments."""
+    device = getattr(env, "device_episodes", False)
+    if device and ((action_fn is None and env.episode_net_supported(net)) or not env.host_step):
+        r = EpisodeKernelRunner(ctx, net, env, **kw)
+    else:
+        r = RolloutRunner(ctx, net, env, **kw)
+    r.action_fn = action_fn
+    return r

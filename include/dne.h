@@ -184,6 +184,27 @@ int dne_cartpole_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_
                           int n_members, const double* d_init_state, int max_steps,
                           float* d_returns, int32_t* d_lengths, double* d_final_state, void* stream);
 
+/* Pendulum-v1 (gymnasium classic_control pendulum.py, DESIGN.md 3.6) episodes run entirely on the device, one per member,
+ * for MujocoPolicy 'continuous:' nets.  Weights as dne_cartpole_episodes; initial state d_init_state[m] = (th, thdot)
+ * (float64); exactly max_steps (1..200) steps, there is no termination.  Per step: observation float32(cos th, sin th,
+ * thdot); layer input clip((o - mean) / std, -5, 5) with d_ob_mean / d_ob_std (both or neither, as
+ * dne_perturb_forward_mlp); fp32 dense forward (sequential fmaf per output, then + bias; tanh / ReLU hidden layers,
+ * linear head); action = head + d_ac_noise[m][step] (nullable [n][max_steps][1], already scaled); the float64 step.
+ * Outputs: d_returns / d_signreturns float[n] (float32 rewards summed in float64 in step order, rounded once),
+ * d_lengths int32[n] (= max_steps), d_final_state double[n][2] (nullable: the 'final' behaviour characterisation),
+ * d_ob_sum / d_ob_sumsq double[n][3] (both or neither: per-member float64 sums of the unnormalised observations fed to
+ * the forward, dne_ob_stat_accumulate's formula, in step order).  Enqueued on `stream`, no host sync.
+ * Supported nets: 1..DNE_MAX_LAYERS dense layers of any width, DNE_OB_VECTOR with ob_dim 3, n_out 1, tanh or ReLU hidden layers, a
+ * linear head, no batch norm, and one member's weights plus two activation buffers in one CTA's shared memory (227 KB:
+ * hidden [200, 200] runs, [256, 256] does not); anything else returns DNE_ERR_UNSUP with the reason in dne_last_error().
+ * dne_pendulum_net_supported answers the same question without launching (0 or DNE_ERR_UNSUP). */
+int dne_pendulum_net_supported(const dne_net_desc* net);
+int dne_pendulum_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                          const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx, int n_members,
+                          const double* d_init_state, int max_steps, const float* d_ob_mean, const float* d_ob_std,
+                          const float* d_ac_noise, float* d_returns, float* d_signreturns, int32_t* d_lengths,
+                          double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, void* stream);
+
 /* Observation statistics of the running normaliser (es.py:356-363 rollout_and_update_ob_stat; RunningStat es.py:26-48):
  * adds the observations d_obs[slot, :] (float32 [*, ob_dim], the unnormalised vectors fed to this tick's forward) of the m
  * listed slots -- the slots whose episode was sampled with probability calc_obstat_prob -- into float64 running sums

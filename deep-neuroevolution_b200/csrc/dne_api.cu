@@ -455,6 +455,36 @@ extern "C" int dne_perturb_forward_conv(dne_ctx* ctx, const dne_net_desc* net, c
                         nullptr, nullptr, d_vbn, d_actions, d_logits, d_ws, ws_bytes, stream);
 }
 
+// The part of dne_cartpole_episodes / dne_discrete_episodes after their argument checks; errors are prefixed with `fn`.
+static int discrete_episodes(const char* fn, dne_ctx* ctx, int env, const dne_net_desc* net, const float* d_theta,
+                             const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx, int n_members,
+                             const double* d_init_state, int max_steps, float* d_returns, int32_t* d_lengths,
+                             double* d_final_state, void* stream) {
+    const char* why = "";
+    if (!dne_discrete_net_supported(env, net, &why)) {
+        dne_set_error("%s: net not supported by the episode kernel: %s", fn, why);
+        return DNE_ERR_UNSUP;
+    }
+    if (net->num_params > ctx->noise_count) {
+        dne_set_error("%s: net larger than the noise table", fn);
+        return DNE_ERR_ARG;
+    }
+    if (n_members == 0) return DNE_OK;
+    const int rc = dne_launch_discrete_episodes(env, net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx, n_members,
+                                                d_init_state, max_steps, d_returns, d_lengths, d_final_state,
+                                                (cudaStream_t)stream);
+    if (rc) {
+        dne_set_error("%s: launch setup failed (%d)", fn, rc);
+        return rc;
+    }
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        dne_set_error("%s: kernel launch -> %s", fn, cudaGetErrorString(e));
+        return DNE_ERR_CUDA;
+    }
+    return DNE_OK;
+}
+
 extern "C" int dne_cartpole_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
                                      const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
                                      int n_members, const double* d_init_state, int max_steps, float* d_returns,
@@ -463,22 +493,22 @@ extern "C" int dne_cartpole_episodes(dne_ctx* ctx, const dne_net_desc* net, cons
     DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_lengths, "null pointer");
     DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
     DNE_CHECK_ARG(max_steps >= 1, "max_steps < 1");
-    const char* why = "";
-    if (!dne_cartpole_net_supported(net, &why)) {
-        dne_set_error("dne_cartpole_episodes: net not supported by the episode kernel: %s", why);
-        return DNE_ERR_UNSUP;
-    }
-    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
-    if (n_members == 0) return DNE_OK;
-    const int rc = dne_launch_cartpole_episodes(net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx, n_members,
-                                                d_init_state, max_steps, d_returns, d_lengths, d_final_state,
-                                                (cudaStream_t)stream);
-    if (rc) {
-        dne_set_error("dne_cartpole_episodes: launch setup failed (%d)", rc);
-        return rc;
-    }
-    DNE_LAUNCH_CHECK();
-    return DNE_OK;
+    return discrete_episodes("dne_cartpole_episodes", ctx, DNE_EPISODE_CARTPOLE, net, d_theta, d_noise_idx, d_scale,
+                             d_theta_idx, n_members, d_init_state, max_steps, d_returns, d_lengths, d_final_state, stream);
+}
+
+extern "C" int dne_discrete_episodes(dne_ctx* ctx, int env, const dne_net_desc* net, const float* d_theta,
+                                     const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                     int n_members, const double* d_init_state, int max_steps, float* d_returns,
+                                     int32_t* d_lengths, double* d_final_state, void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    const int limit = dne_discrete_time_limit(env);
+    DNE_CHECK_ARG(limit > 0, "env is not a DNE_EPISODE_* task");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_lengths, "null pointer");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1 && max_steps <= limit, "max_steps outside 1..the task's TimeLimit");
+    return discrete_episodes("dne_discrete_episodes", ctx, env, net, d_theta, d_noise_idx, d_scale, d_theta_idx, n_members,
+                             d_init_state, max_steps, d_returns, d_lengths, d_final_state, stream);
 }
 
 static int pendulum_net_check(const dne_net_desc* net, const char* fn) {

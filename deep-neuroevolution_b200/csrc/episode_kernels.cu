@@ -1,10 +1,10 @@
 // episode_kernels.cu -- whole episodes of a device-resident environment in one launch.
 //
-// CartPole-v1 and Pendulum-v1 (gym classic_control): the policy has a few hundred to a few tens of thousands of
-// parameters and the environment step is a few dozen flops, so the per-tick runner (one forward launch + a device -> host
-// -> device round trip per step) would spend nearly all its time on overhead.  Here a group of threads runs one member's
-// episode from reset to the end: it builds the member's weights once in shared memory, then loops observation -> dense
-// forward -> action -> environment step on the device.
+// CartPole-v1, Acrobot-v1, MountainCar-v0 and Pendulum-v1 (gym classic_control): the policy has a few hundred to a few
+// tens of thousands of parameters and the environment step is a few dozen to a few hundred flops, so the per-tick runner
+// (one forward launch + a device -> host -> device round trip per step) would spend nearly all its time on overhead.  Here a
+// group of threads runs one member's episode from reset to the end: it builds the member's weights once in shared memory,
+// then loops observation -> dense forward -> action -> environment step on the device.
 //
 // Numerics contract (DESIGN.md 3.5, 3.6):
 //   * weights w = fl(theta[row] + fl(scale * noise[idx + j])) -- the same rounding as every other forward of the engine;
@@ -17,10 +17,9 @@
 #include "forward.cuh"
 #include <math_constants.h>
 
-constexpr int EP_WARPS = 8;                 // CartPole: members per CTA (one per warp)
-constexpr int EP_MAX_WIDTH = 32;            // CartPole: every layer width fits one warp: lane j owns output j
-constexpr int CARTPOLE_MAX_LAYERS = 4;
-constexpr int CARTPOLE_OB_DIM = 4, CARTPOLE_ACTIONS = 2;
+constexpr int EP_WARPS = 8;                 // discrete tasks: members per CTA (one per warp)
+constexpr int EP_MAX_WIDTH = 32;            // discrete tasks: every layer width fits one warp: lane j owns output j
+constexpr int DISCRETE_MAX_LAYERS = 4;
 #define EP_STR2(x) #x
 #define EP_STR(x) EP_STR2(x)
 
@@ -65,7 +64,7 @@ __device__ __forceinline__ void build_member_weights(float* w, const EpisodeNet&
 static bool episode_net_common(const dne_net_desc* net, int max_layers, int ob_dim, int n_out, const char* ob_why,
                                const char* out_why, const char** why) {
     if (net->n_layers < 1 || net->n_layers > max_layers) {
-        *why = max_layers == CARTPOLE_MAX_LAYERS ? "needs 1..4 layers" : "needs 1.." EP_STR(DNE_MAX_LAYERS) " layers";
+        *why = max_layers == DISCRETE_MAX_LAYERS ? "needs 1..4 layers" : "needs 1.." EP_STR(DNE_MAX_LAYERS) " layers";
         return false;
     }
     if (net->ob_kind != DNE_OB_VECTOR) { *why = "needs vector observations (DNE_OB_VECTOR)"; return false; }
@@ -89,12 +88,222 @@ static bool episode_net_common(const dne_net_desc* net, int max_layers, int ob_d
     return true;
 }
 
-// Which nets the fused CartPole kernel runs: dense layers only (<= 4, every width <= 32), vector observations of dimension
-// 4, 2 outputs, ReLU hidden layers, no activation on the head, no batch norm.  On failure `why` names the reason.
-bool dne_cartpole_net_supported(const dne_net_desc* net, const char** why) {
-    if (!episode_net_common(net, CARTPOLE_MAX_LAYERS, CARTPOLE_OB_DIM, CARTPOLE_ACTIONS,
-                            "CartPole observations have ob_dim 4", "CartPole has 2 actions (n_out 2)", why))
-        return false;
+// ---- discrete-action tasks: CartPole-v1, Acrobot-v1, MountainCar-v0 ---------------------------------------------------
+// One warp per member; every lane keeps the whole float64 state and steps it (the step is warp-uniform).  A task type
+// supplies STATE_DIM, OB_DIM (<= 32), ACTIONS (<= 32), TIME_LIMIT and MIN_CTAS (the kernel's minimum CTAs per SM: as many
+// as its step fits in without spilling), a constructor loading the float64 state, store(), ob(k) (observation component k
+// as float32) and step(action, reward) (returns done).  Every reward of these tasks is -1.0, 0.0 or +1.0, so their float64
+// sum in step order is an exact integer: step() reports the reward as that integer and the kernel sums integers.
+
+// one CartPole-v1 step (gym cartpole.py), left-to-right products, explicit rounding
+struct CartPoleTask {
+    static constexpr int STATE_DIM = 4, OB_DIM = 4, ACTIONS = 2, TIME_LIMIT = 500;
+    // 6 CTAs (48 member warps) per SM: 40 registers, no spills (the 40-byte stack frame is the local array of double
+    // sin / cos's slow-path argument reduction).  The loop is latency bound, so resident warps are what hides it; 8 CTAs
+    // per SM (32 registers) spills.
+    static constexpr int MIN_CTAS = 6;
+    static constexpr const char* OB_WHY = "CartPole observations have ob_dim 4";
+    static constexpr const char* OUT_WHY = "CartPole has 2 actions (n_out 2)";
+    double x, x_dot, th, th_dot;
+    // gym derives these from its parameters: total_mass = masspole + masscart, polemass_length = masspole * length,
+    // theta_threshold_radians = 12 * 2 * math.pi / 360
+    double total_mass, polemass_length, theta_threshold;
+
+    __device__ __forceinline__ explicit CartPoleTask(const double* s) : x(s[0]), x_dot(s[1]), th(s[2]), th_dot(s[3]) {
+        total_mass = __dadd_rn(0.1, 1.0);
+        polemass_length = __dmul_rn(0.1, 0.5);
+        theta_threshold = __ddiv_rn(__dmul_rn(24.0, CUDART_PI), 360.0);
+    }
+    __device__ __forceinline__ void store(double* s) const {
+        s[0] = x;
+        s[1] = x_dot;
+        s[2] = th;
+        s[3] = th_dot;
+    }
+    __device__ __forceinline__ float ob(int k) const {       // float32(state)
+        return __double2float_rn(k == 0 ? x : k == 1 ? x_dot : k == 2 ? th : th_dot);
+    }
+    __device__ __forceinline__ bool step(int action, int& reward) {
+        const double gravity = 9.8, masspole = 0.1, length = 0.5, force_mag = 10.0, tau = 0.02, x_threshold = 2.4;
+        const double force = action == 1 ? force_mag : -force_mag;
+        const double c = cos(th), sn = sin(th);
+        // temp = (force + polemass_length * theta_dot**2 * sintheta) / total_mass
+        const double temp = __ddiv_rn(__dadd_rn(force, __dmul_rn(__dmul_rn(polemass_length, __dmul_rn(th_dot, th_dot)), sn)),
+                                      total_mass);
+        // thetaacc = (gravity * sintheta - costheta * temp) / (length * (4.0 / 3.0 - masspole * costheta**2 / total_mass))
+        const double den = __dmul_rn(length, __dsub_rn(__ddiv_rn(4.0, 3.0),
+                                                       __ddiv_rn(__dmul_rn(masspole, __dmul_rn(c, c)), total_mass)));
+        const double thetaacc = __ddiv_rn(__dsub_rn(__dmul_rn(gravity, sn), __dmul_rn(c, temp)), den);
+        // xacc = temp - polemass_length * thetaacc * costheta / total_mass
+        const double xacc = __dsub_rn(temp, __ddiv_rn(__dmul_rn(__dmul_rn(polemass_length, thetaacc), c), total_mass));
+        x = __dadd_rn(x, __dmul_rn(tau, x_dot));                     // Euler, gym's order
+        x_dot = __dadd_rn(x_dot, __dmul_rn(tau, xacc));
+        th = __dadd_rn(th, __dmul_rn(tau, th_dot));
+        th_dot = __dadd_rn(th_dot, __dmul_rn(tau, thetaacc));
+        reward = 1;                                                   // the terminating step included
+        return x < -x_threshold || x > x_threshold || th < -theta_threshold || th > theta_threshold;
+    }
+};
+
+// Acrobot-v1 (gymnasium acrobot.py, "book" dynamics, no torque noise): state (theta1, theta2, dtheta1, dtheta2), one RK4
+// step of dt = 0.2 per action, torque [-1, 0, +1][action].  DESIGN.md 3.5 writes out the operation order.
+constexpr double ACRO_M1 = 1.0, ACRO_M2 = 1.0, ACRO_L1 = 1.0, ACRO_LC1 = 0.5, ACRO_LC2 = 0.5, ACRO_I1 = 1.0,
+                 ACRO_I2 = 1.0, ACRO_G = 9.8, ACRO_DT = 0.2;
+// gym's wrap() loops for ever on an angle it cannot bring into [-pi, pi]; the kernel gives up after this many turns (a
+// state the dynamics reach from any reset moves far less than one turn per step)
+constexpr int ACRO_WRAP_MAX_TURNS = 4096;
+
+// _dsdt: the time derivative (ddtheta1, ddtheta2) of the velocities under torque `a` (the angles' derivatives are the
+// velocities themselves, the torque's is 0)
+__device__ __forceinline__ void acrobot_accel(double th1, double th2, double dth1, double dth2, double a, double& ddth1,
+                                              double& ddth2) {
+    const double m1 = ACRO_M1, m2 = ACRO_M2, l1 = ACRO_L1, lc1 = ACRO_LC1, lc2 = ACRO_LC2, I1 = ACRO_I1, I2 = ACRO_I2,
+                 g = ACRO_G, pi = CUDART_PI;
+    const double ct2 = cos(th2), st2 = sin(th2);
+    // d1 = m1 * lc1**2 + m2 * (l1**2 + lc2**2 + 2 * l1 * lc2 * cos(theta2)) + I1 + I2
+    const double d1 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m1, __dmul_rn(lc1, lc1)),
+                                                    __dmul_rn(m2, __dadd_rn(__dadd_rn(__dmul_rn(l1, l1), __dmul_rn(lc2, lc2)),
+                                                                            __dmul_rn(__dmul_rn(__dmul_rn(2.0, l1), lc2), ct2)))),
+                                          I1),
+                                I2);
+    // d2 = m2 * (lc2**2 + l1 * lc2 * cos(theta2)) + I2
+    const double d2 = __dadd_rn(__dmul_rn(m2, __dadd_rn(__dmul_rn(lc2, lc2), __dmul_rn(__dmul_rn(l1, lc2), ct2))), I2);
+    // phi2 = m2 * lc2 * g * cos(theta1 + theta2 - pi / 2.0)
+    const double phi2 = __dmul_rn(__dmul_rn(__dmul_rn(m2, lc2), g), cos(__dsub_rn(__dadd_rn(th1, th2), __ddiv_rn(pi, 2.0))));
+    // phi1 = -m2 * l1 * lc2 * dtheta2**2 * sin(theta2) - 2 * m2 * l1 * lc2 * dtheta2 * dtheta1 * sin(theta2)
+    //        + (m1 * lc1 + m2 * l1) * g * cos(theta1 - pi / 2) + phi2
+    const double p1 = __dmul_rn(__dmul_rn(__dmul_rn(__dmul_rn(-m2, l1), lc2), __dmul_rn(dth2, dth2)), st2);
+    const double p2 = __dmul_rn(__dmul_rn(__dmul_rn(__dmul_rn(__dmul_rn(__dmul_rn(2.0, m2), l1), lc2), dth2), dth1), st2);
+    const double p3 = __dmul_rn(__dmul_rn(__dadd_rn(__dmul_rn(m1, lc1), __dmul_rn(m2, l1)), g),
+                                cos(__dsub_rn(th1, __ddiv_rn(pi, 2.0))));
+    const double phi1 = __dadd_rn(__dadd_rn(__dsub_rn(p1, p2), p3), phi2);
+    // ddtheta2 = (a + d2 / d1 * phi1 - m2 * l1 * lc2 * dtheta1**2 * sin(theta2) - phi2) / (m2 * lc2**2 + I2 - d2**2 / d1)
+    const double num = __dsub_rn(__dsub_rn(__dadd_rn(a, __dmul_rn(__ddiv_rn(d2, d1), phi1)),
+                                           __dmul_rn(__dmul_rn(__dmul_rn(__dmul_rn(m2, l1), lc2), __dmul_rn(dth1, dth1)), st2)),
+                                 phi2);
+    const double den = __dsub_rn(__dadd_rn(__dmul_rn(m2, __dmul_rn(lc2, lc2)), I2), __ddiv_rn(__dmul_rn(d2, d2), d1));
+    ddth2 = __ddiv_rn(num, den);
+    // ddtheta1 = -(d2 * ddtheta2 + phi1) / d1
+    ddth1 = __ddiv_rn(-__dadd_rn(__dmul_rn(d2, ddth2), phi1), d1);
+}
+
+struct AcrobotTask {
+    static constexpr int STATE_DIM = 4, OB_DIM = 6, ACTIONS = 3, TIME_LIMIT = 500;
+    static constexpr int MIN_CTAS = 4;            // 64 registers, no spills; 5 CTAs per SM (48 registers) spills
+    static constexpr const char* OB_WHY = "Acrobot observations have ob_dim 6";
+    static constexpr const char* OUT_WHY = "Acrobot has 3 actions (n_out 3)";
+    double th1, th2, dth1, dth2;
+
+    __device__ __forceinline__ explicit AcrobotTask(const double* s) : th1(s[0]), th2(s[1]), dth1(s[2]), dth2(s[3]) {}
+    __device__ __forceinline__ void store(double* s) const {
+        s[0] = th1;
+        s[1] = th2;
+        s[2] = dth1;
+        s[3] = dth2;
+    }
+    __device__ __forceinline__ float ob(int k) const {       // float32([cos th1, sin th1, cos th2, sin th2, dth1, dth2])
+        const double a = k < 2 ? th1 : th2;
+        return __double2float_rn(k == 4 ? dth1 : k == 5 ? dth2 : (k & 1) ? sin(a) : cos(a));
+    }
+    static __device__ __forceinline__ double wrap(double x) {                // gym's wrap(x, -pi, pi)
+        const double m = -CUDART_PI, M = CUDART_PI, diff = __dsub_rn(M, m);
+        for (int i = 0; i < ACRO_WRAP_MAX_TURNS && x > M; ++i) x = __dsub_rn(x, diff);
+        for (int i = 0; i < ACRO_WRAP_MAX_TURNS && x < m; ++i) x = __dadd_rn(x, diff);
+        return x;
+    }
+    static __device__ __forceinline__ double bound(double x, double B) {      // gym's bound(x, -B, B) = min(max(x, -B), B)
+        x = -B > x ? -B : x;
+        return B < x ? B : x;
+    }
+    __device__ __forceinline__ bool step(int action, int& reward) {
+        const double a = (double)(action - 1);                        // AVAIL_TORQUE = [-1.0, 0.0, +1]
+        const double dt = ACRO_DT, dt2 = __ddiv_rn(dt, 2.0);
+        // rk4: k1 = f(y0), k2 = f(y0 + dt2 * k1), k3 = f(y0 + dt2 * k2), k4 = f(y0 + dt * k3);
+        // y0 + dt / 6.0 * (k1 + 2 * k2 + 2 * k3 + k4), the sum accumulated left to right as it is built
+        double k0, k1, k2, k3;                                        // one stage's derivative
+        double s0, s1, s2, s3;                                        // k1 + 2 * k2 + ..., so far
+        acrobot_accel(th1, th2, dth1, dth2, a, k2, k3);
+        k0 = dth1;
+        k1 = dth2;
+        s0 = k0, s1 = k1, s2 = k2, s3 = k3;
+#pragma unroll 1
+        for (int stage = 1; stage < 4; ++stage) {
+            const double h = stage < 3 ? dt2 : dt;
+            const double y0 = __dadd_rn(th1, __dmul_rn(h, k0)), y1 = __dadd_rn(th2, __dmul_rn(h, k1));
+            const double y2 = __dadd_rn(dth1, __dmul_rn(h, k2)), y3 = __dadd_rn(dth2, __dmul_rn(h, k3));
+            acrobot_accel(y0, y1, y2, y3, a, k2, k3);
+            k0 = y2;
+            k1 = y3;
+            const double c = stage < 3 ? 2.0 : 1.0;
+            s0 = __dadd_rn(s0, __dmul_rn(c, k0));
+            s1 = __dadd_rn(s1, __dmul_rn(c, k1));
+            s2 = __dadd_rn(s2, __dmul_rn(c, k2));
+            s3 = __dadd_rn(s3, __dmul_rn(c, k3));
+        }
+        const double d6 = __ddiv_rn(dt, 6.0);
+        th1 = wrap(__dadd_rn(th1, __dmul_rn(d6, s0)));
+        th2 = wrap(__dadd_rn(th2, __dmul_rn(d6, s1)));
+        dth1 = bound(__dadd_rn(dth1, __dmul_rn(d6, s2)), __dmul_rn(4.0, CUDART_PI));     // MAX_VEL_1 = 4 * pi
+        dth2 = bound(__dadd_rn(dth2, __dmul_rn(d6, s3)), __dmul_rn(9.0, CUDART_PI));     // MAX_VEL_2 = 9 * pi
+        // _terminal: -cos(s[0]) - cos(s[1] + s[0]) > 1.0; reward -1, 0 on the terminating step
+        const bool done = __dsub_rn(-cos(th1), cos(__dadd_rn(th2, th1))) > 1.0;
+        reward = done ? 0 : -1;
+        return done;
+    }
+};
+
+// MountainCar-v0 (gymnasium mountain_car.py): state (position, velocity), reward -1 on every step.
+struct MountainCarTask {
+    static constexpr int STATE_DIM = 2, OB_DIM = 2, ACTIONS = 3, TIME_LIMIT = 200;
+    static constexpr int MIN_CTAS = 6;            // 40 registers, no spills; 8 CTAs per SM (32 registers) spills
+    static constexpr const char* OB_WHY = "MountainCar observations have ob_dim 2";
+    static constexpr const char* OUT_WHY = "MountainCar has 3 actions (n_out 3)";
+    double x, v;
+
+    __device__ __forceinline__ explicit MountainCarTask(const double* s) : x(s[0]), v(s[1]) {}
+    __device__ __forceinline__ void store(double* s) const {
+        s[0] = x;
+        s[1] = v;
+    }
+    __device__ __forceinline__ float ob(int k) const { return __double2float_rn(k == 0 ? x : v); }
+    __device__ __forceinline__ bool step(int action, int& reward) {
+        const double force = 0.001, gravity = 0.0025, max_speed = 0.07, min_position = -1.2, max_position = 0.6;
+        // velocity += (action - 1) * force + math.cos(3 * position) * (-gravity); np.clip(velocity, -max_speed, max_speed)
+        v = __dadd_rn(v, __dadd_rn(__dmul_rn((double)(action - 1), force), __dmul_rn(cos(__dmul_rn(3.0, x)), -gravity)));
+        v = v < -max_speed ? -max_speed : (v > max_speed ? max_speed : v);
+        // position += velocity; np.clip(position, min_position, max_position)
+        x = __dadd_rn(x, v);
+        x = x < min_position ? min_position : (x > max_position ? max_position : x);
+        if (x == min_position && v < 0.0) v = 0.0;
+        reward = -1;                                                  // the terminating step included
+        return x >= 0.5 && v >= 0.0;                                  // goal_position 0.5, goal_velocity 0
+    }
+};
+
+// argmax over the logits held by lanes 0..A-1: the first NaN if any logit is NaN, otherwise the first maximum
+// (dense_small_kernel's rule).  For A = 2 this is (y0 != y0) ? 0 : ((y1 > y0 || y1 != y1) ? 1 : 0).
+template <int A>
+__device__ __forceinline__ int warp_argmax(float x) {
+    int best = 0;
+    float bv = __shfl_sync(0xffffffffu, x, 0);
+#pragma unroll
+    for (int j = 1; j < A; ++j) {
+        const float y = __shfl_sync(0xffffffffu, x, j);
+        if (bv == bv && (y > bv || y != y)) {
+            best = j;
+            bv = y;
+        }
+    }
+    return best;
+}
+
+// Which nets the discrete episode kernel runs for task T: dense layers only (<= 4, every width <= 32), vector observations
+// of dimension T::OB_DIM, T::ACTIONS outputs, ReLU hidden layers, no activation on the head, no batch norm.  On failure
+// `why` names the reason.
+template <class T>
+static bool discrete_net_supported(const dne_net_desc* net, const char** why) {
+    static_assert(T::OB_DIM <= EP_MAX_WIDTH && T::ACTIONS <= EP_MAX_WIDTH, "one lane per observation and per action");
+    if (!episode_net_common(net, DISCRETE_MAX_LAYERS, T::OB_DIM, T::ACTIONS, T::OB_WHY, T::OUT_WHY, why)) return false;
     for (int l = 0; l < net->n_layers; ++l) {
         const dne_layer_desc& L = net->layers[l];
         const bool head = (l == net->n_layers - 1);
@@ -104,41 +313,14 @@ bool dne_cartpole_net_supported(const dne_net_desc* net, const char** why) {
             return false;
         }
     }
-    // the largest net the rules above allow (4 layers of width 32) has 3328 parameters
+    // the largest net the rules above allow (4 layers of width 32) has at most 3328 parameters
     if (net->num_params > 4096) { *why = "num_params too large for the shared-memory weights"; return false; }
     return true;
 }
 
-// one CartPole-v1 step (gym cartpole.py), left-to-right products, explicit rounding
-struct CartPole {
-    double x, x_dot, th, th_dot;
-};
-__device__ __forceinline__ bool cartpole_step(CartPole& s, int action, double total_mass, double polemass_length,
-                                              double theta_threshold) {
-    const double gravity = 9.8, masspole = 0.1, length = 0.5, force_mag = 10.0, tau = 0.02, x_threshold = 2.4;
-    const double force = action == 1 ? force_mag : -force_mag;
-    const double c = cos(s.th), sn = sin(s.th);
-    // temp = (force + polemass_length * theta_dot**2 * sintheta) / total_mass
-    const double temp = __ddiv_rn(__dadd_rn(force, __dmul_rn(__dmul_rn(polemass_length, __dmul_rn(s.th_dot, s.th_dot)), sn)),
-                                  total_mass);
-    // thetaacc = (gravity * sintheta - costheta * temp) / (length * (4.0 / 3.0 - masspole * costheta**2 / total_mass))
-    const double den = __dmul_rn(length, __dsub_rn(__ddiv_rn(4.0, 3.0),
-                                                   __ddiv_rn(__dmul_rn(masspole, __dmul_rn(c, c)), total_mass)));
-    const double thetaacc = __ddiv_rn(__dsub_rn(__dmul_rn(gravity, sn), __dmul_rn(c, temp)), den);
-    // xacc = temp - polemass_length * thetaacc * costheta / total_mass
-    const double xacc = __dsub_rn(temp, __ddiv_rn(__dmul_rn(__dmul_rn(polemass_length, thetaacc), c), total_mass));
-    s.x = __dadd_rn(s.x, __dmul_rn(tau, s.x_dot));                 // Euler, gym's order
-    s.x_dot = __dadd_rn(s.x_dot, __dmul_rn(tau, xacc));
-    s.th = __dadd_rn(s.th, __dmul_rn(tau, s.th_dot));
-    s.th_dot = __dadd_rn(s.th_dot, __dmul_rn(tau, thetaacc));
-    return s.x < -x_threshold || s.x > x_threshold || s.th < -theta_threshold || s.th > theta_threshold;
-}
-
-// 6 CTAs (48 member warps) per SM: 40 registers, no spills (the 40-byte stack frame is the local array of double
-// sin / cos's slow-path argument reduction).  The loop is latency bound, so resident warps are what hides it; 8 CTAs per SM
-// (32 registers) spills.
-__global__ void __launch_bounds__(EP_WARPS * 32, 6)
-cartpole_episode_kernel(EpisodeNet net, const float* __restrict__ theta, const float* __restrict__ noise,
+template <class T>
+__global__ void __launch_bounds__(EP_WARPS * 32, T::MIN_CTAS)
+discrete_episode_kernel(EpisodeNet net, const float* __restrict__ theta, const float* __restrict__ noise,
                         const int64_t* __restrict__ noise_idx, const float* __restrict__ scale,
                         const int32_t* __restrict__ theta_idx, int n_members, const double* __restrict__ init_state,
                         int max_steps, float* __restrict__ returns, int32_t* __restrict__ lengths,
@@ -152,23 +334,14 @@ cartpole_episode_kernel(EpisodeNet net, const float* __restrict__ theta, const f
     build_member_weights(w, net, theta, noise, noise_idx, scale, theta_idx, m, lane, 32);
     __syncwarp();
 
-    // gym derives these from its parameters: total_mass = masspole + masscart, polemass_length = masspole * length,
-    // theta_threshold_radians = 12 * 2 * math.pi / 360
-    const double total_mass = __dadd_rn(0.1, 1.0);
-    const double polemass_length = __dmul_rn(0.1, 0.5);
-    const double theta_threshold = __ddiv_rn(__dmul_rn(24.0, CUDART_PI), 360.0);
-
-    CartPole st;
-    st.x = init_state[4 * m + 0];
-    st.x_dot = init_state[4 * m + 1];
-    st.th = init_state[4 * m + 2];
-    st.th_dot = init_state[4 * m + 3];
+    T env(init_state + (int64_t)T::STATE_DIM * m);
+    int ret = 0;                                                  // the sum of the rewards, exact
     int len = 0;
     bool done = false;
     while (!done && len < max_steps) {
-        // lane k < 4 holds observation component k (every lane keeps the full state: the step is warp-uniform)
-        const double sk = lane == 0 ? st.x : lane == 1 ? st.x_dot : lane == 2 ? st.th : st.th_dot;
-        float x = lane < CARTPOLE_OB_DIM ? __double2float_rn(sk) : 0.0f;
+        // lane k < OB_DIM holds observation component k (the others compute the last one and drop it: no branch)
+        const float o = env.ob(lane < T::OB_DIM ? lane : T::OB_DIM - 1);
+        float x = lane < T::OB_DIM ? o : 0.0f;
         for (int l = 0; l < net.n_layers; ++l) {
             const int K = net.cin[l], N = net.cout[l];
             const float* wl = w + net.off_w[l];
@@ -179,37 +352,70 @@ cartpole_episode_kernel(EpisodeNet net, const float* __restrict__ theta, const f
             if (l + 1 < net.n_layers) y = fmaxf(y, 0.0f);                 // ReLU (hidden layers)
             x = lane < N ? y : 0.0f;
         }
-        const float y0 = __shfl_sync(0xffffffffu, x, 0), y1 = __shfl_sync(0xffffffffu, x, 1);
-        const int action = (y0 != y0) ? 0 : ((y1 > y0 || y1 != y1) ? 1 : 0);   // first max, NaN is the max
-        done = cartpole_step(st, action, total_mass, polemass_length, theta_threshold);
+        int r;
+        done = env.step(warp_argmax<T::ACTIONS>(x), r);
+        ret += r;
         ++len;
     }
     if (lane == 0) {
-        returns[m] = (float)len;                                  // reward 1.0 on every step, the terminating one included
+        returns[m] = (float)ret;                                  // |ret| <= 500: exact
         lengths[m] = len;
-        if (final_state) {
-            final_state[4 * m + 0] = st.x;
-            final_state[4 * m + 1] = st.x_dot;
-            final_state[4 * m + 2] = st.th;
-            final_state[4 * m + 3] = st.th_dot;
-        }
+        if (final_state) env.store(final_state + (int64_t)T::STATE_DIM * m);
     }
 }
 
-int dne_launch_cartpole_episodes(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,
-                                 const float* scale, const int32_t* theta_idx, int n_members, const double* init_state,
-                                 int max_steps, float* returns, int32_t* lengths, double* final_state, cudaStream_t st) {
+template <class T>
+static int launch_discrete(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,
+                           const float* scale, const int32_t* theta_idx, int n_members, const double* init_state,
+                           int max_steps, float* returns, int32_t* lengths, double* final_state, cudaStream_t st) {
     const EpisodeNet en = make_episode_net(net);
     const size_t smem = (size_t)EP_WARPS * en.P_pad * sizeof(float);
     if (smem > 48 * 1024) {
-        const cudaError_t e = cudaFuncSetAttribute(cartpole_episode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        const cudaError_t e = cudaFuncSetAttribute(discrete_episode_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)smem);
         if (e != cudaSuccess) return DNE_ERR_CUDA;
     }
     const unsigned grid = (unsigned)((n_members + EP_WARPS - 1) / EP_WARPS);
-    cartpole_episode_kernel<<<grid, EP_WARPS * 32, smem, st>>>(en, theta, noise, noise_idx, scale, theta_idx, n_members,
-                                                               init_state, max_steps, returns, lengths, final_state);
+    discrete_episode_kernel<T><<<grid, EP_WARPS * 32, smem, st>>>(en, theta, noise, noise_idx, scale, theta_idx, n_members,
+                                                                  init_state, max_steps, returns, lengths, final_state);
     DNE_LAUNCHED(1);
     return DNE_OK;
+}
+
+int dne_discrete_time_limit(int env) {
+    switch (env) {
+        case DNE_EPISODE_CARTPOLE: return CartPoleTask::TIME_LIMIT;
+        case DNE_EPISODE_ACROBOT: return AcrobotTask::TIME_LIMIT;
+        case DNE_EPISODE_MOUNTAINCAR: return MountainCarTask::TIME_LIMIT;
+        default: return 0;
+    }
+}
+
+bool dne_discrete_net_supported(int env, const dne_net_desc* net, const char** why) {
+    switch (env) {
+        case DNE_EPISODE_CARTPOLE: return discrete_net_supported<CartPoleTask>(net, why);
+        case DNE_EPISODE_ACROBOT: return discrete_net_supported<AcrobotTask>(net, why);
+        case DNE_EPISODE_MOUNTAINCAR: return discrete_net_supported<MountainCarTask>(net, why);
+        default: *why = "unknown environment"; return false;
+    }
+}
+
+int dne_launch_discrete_episodes(int env, const dne_net_desc* net, const float* theta, const float* noise,
+                                 const int64_t* noise_idx, const float* scale, const int32_t* theta_idx, int n_members,
+                                 const double* init_state, int max_steps, float* returns, int32_t* lengths,
+                                 double* final_state, cudaStream_t st) {
+    switch (env) {
+        case DNE_EPISODE_CARTPOLE:
+            return launch_discrete<CartPoleTask>(net, theta, noise, noise_idx, scale, theta_idx, n_members, init_state,
+                                                 max_steps, returns, lengths, final_state, st);
+        case DNE_EPISODE_ACROBOT:
+            return launch_discrete<AcrobotTask>(net, theta, noise, noise_idx, scale, theta_idx, n_members, init_state,
+                                                max_steps, returns, lengths, final_state, st);
+        case DNE_EPISODE_MOUNTAINCAR:
+            return launch_discrete<MountainCarTask>(net, theta, noise, noise_idx, scale, theta_idx, n_members, init_state,
+                                                    max_steps, returns, lengths, final_state, st);
+        default: return DNE_ERR_ARG;
+    }
 }
 
 // ---- Pendulum-v1 ------------------------------------------------------------------------------------------------------

@@ -94,11 +94,14 @@ int dne_launch_dense_layer(const dne_ctx* ctx, const SlotArgs& sa, const dne_lay
 void dne_launch_ob_norm(const float* obs, const float* mean, const float* stdv, int64_t total, int dim, float* out,
                         cudaStream_t st);
 
-// episode_kernels.cu: whole CartPole-v1 episodes on the device (dne_cartpole_episodes)
-bool dne_cartpole_net_supported(const dne_net_desc* net, const char** why);
-int dne_launch_cartpole_episodes(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,
-                                 const float* scale, const int32_t* theta_idx, int n_members, const double* init_state,
-                                 int max_steps, float* returns, int32_t* lengths, double* final_state, cudaStream_t st);
+// episode_kernels.cu: whole episodes of the DNE_EPISODE_* discrete-action tasks on the device (dne_discrete_episodes,
+// dne_cartpole_episodes); dne_discrete_time_limit is 0 for an unknown task
+int dne_discrete_time_limit(int env);
+bool dne_discrete_net_supported(int env, const dne_net_desc* net, const char** why);
+int dne_launch_discrete_episodes(int env, const dne_net_desc* net, const float* theta, const float* noise,
+                                 const int64_t* noise_idx, const float* scale, const int32_t* theta_idx, int n_members,
+                                 const double* init_state, int max_steps, float* returns, int32_t* lengths,
+                                 double* final_state, cudaStream_t st);
 // episode_kernels.cu: whole Pendulum-v1 episodes on the device (dne_pendulum_episodes)
 bool dne_pendulum_net_supported(const dne_net_desc* net, const char** why);
 int dne_launch_pendulum_episodes(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,

@@ -19,6 +19,7 @@ CONV, DENSE = 0, 1
 ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
 BN_NONE, BN_TF, BN_GPU = 0, 1, 2
 OB_ATARI_U8, OB_VECTOR = 0, 1
+EPISODE_CARTPOLE, EPISODE_ACROBOT, EPISODE_MOUNTAINCAR = 0, 1, 2
 
 
 class LayerDesc(C.Structure):
@@ -52,6 +53,7 @@ _SIGS = {
                                 C.c_size_t, _P],
     "dne_ob_stat_accumulate": [_P, C.c_int, _P, C.c_int, _P, _P, _P],
     "dne_cartpole_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P],
+    "dne_discrete_episodes": [_P, C.c_int, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P],
     "dne_pendulum_net_supported": [C.POINTER(NetDesc)],
     "dne_pendulum_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                               _P, _P, _P],

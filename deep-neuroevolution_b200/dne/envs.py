@@ -9,8 +9,9 @@ Step`` over a batch of ALE instances (gpu_implementation/gym_tensorflow/tf_env.c
 ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so the environment shipped
 here is the synthetic Frostbite-shaped stub the measurement plan names (SURVEY.md 8d): i.i.d. uint8 84x84x4
 observations from a fixed pool, rewards 10*Bernoulli(0.05), fixed or ragged episode lengths.  A real emulator
-plugs in by subclassing ``BatchEnv``.  Two real tasks need no emulator: CartPole-v1 (``CartPoleEnv``) and Pendulum-v1
-(``PendulumEnv``), whose episodes run whole on the device (``dne.rollout.EpisodeKernelRunner``).
+plugs in by subclassing ``BatchEnv``.  Four real tasks need no emulator: CartPole-v1 (``CartPoleEnv``), Acrobot-v1
+(``AcrobotEnv``), MountainCar-v0 (``MountainCarEnv``) and Pendulum-v1 (``PendulumEnv``), whose episodes run whole on the
+device (``dne.rollout.EpisodeKernelRunner``).
 
 An environment with device episodes (``device_episodes = True``) supplies ``state_dim``, ``initial_states(k)``,
 ``episode_net_supported(net)`` and ``launch_episodes(...)``; ``kernel_policy_io`` says whether its kernel also takes
@@ -210,8 +211,8 @@ class SyntheticVectorEnv(BatchEnv):
 def make_env(env_id: str, n_slots: int, seed: int = 0, episode_len=None, allow_synthetic: bool = False, **kw) -> BatchEnv:
     """``gym.make(exp['env_id'])`` (es.py:131) for a whole slot table.
 
-    ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so apart from CartPole-v1 and
-    Pendulum-v1 (``CartPoleEnv``, ``PendulumEnv``, registered in ``ENV_BACKENDS``) the only backends here are the synthetic stubs.  They are returned for the explicit ids ``SyntheticAtari*`` / ``SyntheticVector*``; for a REAL id
+    ALE / gym / MuJoCo are not vendored by the reference and are absent from this image, so apart from CartPole-v1,
+    Acrobot-v1, MountainCar-v0 and Pendulum-v1 (registered in ``ENV_BACKENDS``) the only backends here are the synthetic stubs.  They are returned for the explicit ids ``SyntheticAtari*`` / ``SyntheticVector*``; for a REAL id
     (``FrostbiteNoFrameskip-v4``, ``Humanoid-v1`` ...) they are returned only when the caller opts in
     (``exp['allow_synthetic_env'] = true`` or ``DNE_ALLOW_SYNTHETIC_ENV=1``), with a loud warning -- a run that silently
     optimised random frames while logging and snapshotting like a real one would be worse than an error.  A real emulator
@@ -241,15 +242,39 @@ def make_env(env_id: str, n_slots: int, seed: int = 0, episode_len=None, allow_s
     return env
 
 
-class CartPoleEnv(BatchEnv):
+class DiscreteDeviceEnv(BatchEnv):
+    """Base of gym's discrete-action classic_control tasks whose whole episodes run ON THE DEVICE, one warp per member
+    (``dne_discrete_episodes``, ``dne.rollout.EpisodeKernelRunner``): a subclass supplies the spaces, the time limit,
+    ``state_dim``, its ``DNE_EPISODE_*`` id and ``initial_states(k)``, drawn from one ``RandomState(seed)`` stream that
+    continues across calls, as one gym env reset k times in a row would.  There is no host step."""
+    device_episodes = True
+    host_step = False
+    kernel_policy_io = False       # no observation normalisation, action noise or observation statistics in the kernel
+    episode_env: int = -1          # DNE_EPISODE_*
+
+    def episode_net_supported(self, net) -> bool:
+        return True                # the only path: the kernel itself rejects a net it cannot run
+
+    def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
+                        **_):
+        F.check(F.lib().dne_discrete_episodes(
+            ctx.handle, self.episode_env, C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale),
+            F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ret), F.ptr(d_len), F.ptr(d_fin), F.stream_ptr()))
+        d_sret.copy_(d_ret)        # every reward is -1, 0 or +1: the sign-return is the return
+
+    def _host_stepping(self, *a, **kw):
+        raise NotImplementedError(f"{type(self).__name__} runs whole episodes on the device: use dne.rollout.make_runner "
+                                  "(EpisodeKernelRunner), not the per-tick host reset / step")
+    reset = step = obs_block = get_ram = _host_stepping
+
+
+class CartPoleEnv(DiscreteDeviceEnv):
     """gym's CartPole-v1 (classic_control cartpole.py) for a whole population, stepped ON THE DEVICE: whole episodes run in
     one launch of ``dne_cartpole_episodes`` (``dne.rollout.EpisodeKernelRunner``), so this object only supplies the spaces,
     the time limit, the reset states and the launch.  ``initial_states(k)`` draws k resets ``uniform(-0.05, 0.05, size=4)``
     from one ``RandomState(seed)`` stream that continues across calls, as one gym env reset k times in a row would."""
-    device_episodes = True
-    host_step = False
-    kernel_policy_io = False       # no observation normalisation, action noise or observation statistics in the kernel
     state_dim = 4
+    episode_env = F.EPISODE_CARTPOLE
 
     def __init__(self, n_slots: int, seed: int = 0):
         self.n_slots = int(n_slots)
@@ -264,9 +289,6 @@ class CartPoleEnv(BatchEnv):
         """float64 [k, 4] reset states (gym ``reset``: ``uniform(low=-0.05, high=0.05, size=(4,))`` per episode)."""
         return self.rs.uniform(-0.05, 0.05, size=(int(k), 4))
 
-    def episode_net_supported(self, net) -> bool:
-        return True                # the only path: dne_cartpole_episodes itself rejects a net it cannot run
-
     def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
                         **_):
         F.check(F.lib().dne_cartpole_episodes(
@@ -274,16 +296,65 @@ class CartPoleEnv(BatchEnv):
             F.ptr(d_init), int(limit), F.ptr(d_ret), F.ptr(d_len), F.ptr(d_fin), F.stream_ptr()))
         d_sret.copy_(d_ret)        # every reward is +1: the sign-return is the return
 
-    def _host_stepping(self, *a, **kw):
-        raise NotImplementedError("CartPoleEnv runs whole episodes on the device: use dne.rollout.make_runner "
-                                  "(EpisodeKernelRunner), not the per-tick host reset / step")
-    reset = step = obs_block = get_ram = _host_stepping
-
 
 def _make_cartpole(env_id, n_slots, seed=0, episode_len=None, **kw):
     if episode_len is not None:
         raise ValueError("CartPole-v1 has a fixed 500-step time limit; use the episode cutoff of the config instead")
     return CartPoleEnv(n_slots, seed=seed)
+
+
+class AcrobotEnv(DiscreteDeviceEnv):
+    """gymnasium's Acrobot-v1 (classic_control acrobot.py, "book" dynamics, no torque noise; DESIGN.md 3.5) for a whole
+    population, stepped on the device.  State (theta1, theta2, dtheta1, dtheta2); observation float32([cos theta1,
+    sin theta1, cos theta2, sin theta2, dtheta1, dtheta2]); 3 actions (torque -1, 0, +1); reward -1 per step, 0 on the
+    terminating one; TimeLimit 500.  Resets draw ``uniform(-0.1, 0.1, size=4)`` per episode, rounded to float32 as gym
+    stores them."""
+    state_dim = 4
+    episode_env = F.EPISODE_ACROBOT
+
+    def __init__(self, n_slots: int, seed: int = 0):
+        self.n_slots = int(n_slots)
+        high = np.array([1.0, 1.0, 1.0, 1.0, 4 * np.pi, 9 * np.pi], dtype=np.float32)   # gym's observation_space bounds
+        self.observation_space = Box(-high, high)
+        self.action_space = Discrete(3)
+        self.max_episode_steps = 500                                             # TimeLimit of Acrobot-v1
+        self.rs = np.random.RandomState(seed)
+
+    def initial_states(self, k: int) -> np.ndarray:
+        """float64 [k, 4] reset states."""
+        return self.rs.uniform(-0.1, 0.1, size=(int(k), 4)).astype(np.float32).astype(np.float64)
+
+
+class MountainCarEnv(DiscreteDeviceEnv):
+    """gymnasium's MountainCar-v0 (classic_control mountain_car.py; DESIGN.md 3.5) for a whole population, stepped on the
+    device.  State and observation (position, velocity); 3 actions (push left, none, right); reward -1 on every step; done
+    at position >= 0.5 with velocity >= 0; TimeLimit 200.  Resets draw the position ``uniform(-0.6, -0.4)`` per episode,
+    velocity 0."""
+    state_dim = 2
+    episode_env = F.EPISODE_MOUNTAINCAR
+
+    def __init__(self, n_slots: int, seed: int = 0):
+        self.n_slots = int(n_slots)
+        self.observation_space = Box(np.array([-1.2, -0.07], np.float32), np.array([0.6, 0.07], np.float32))
+        self.action_space = Discrete(3)
+        self.max_episode_steps = 200                                             # TimeLimit of MountainCar-v0
+        self.rs = np.random.RandomState(seed)
+
+    def initial_states(self, k: int) -> np.ndarray:
+        """float64 [k, 2] reset states (position, 0)."""
+        return np.stack([self.rs.uniform(-0.6, -0.4, size=int(k)), np.zeros(int(k))], axis=1)
+
+
+def _fixed_limit_factory(cls, name, limit):
+    def make(env_id, n_slots, seed=0, episode_len=None, **kw):
+        if episode_len is not None:
+            raise ValueError(f"{name} has a fixed {limit}-step time limit; use the episode cutoff of the config instead")
+        return cls(n_slots, seed=seed)
+    return make
+
+
+_make_acrobot = _fixed_limit_factory(AcrobotEnv, "Acrobot-v1", 500)
+_make_mountaincar = _fixed_limit_factory(MountainCarEnv, "MountainCar-v0", 200)
 
 
 class PendulumEnv(BatchEnv):
@@ -364,4 +435,8 @@ ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_
     "CartPole-v1": _make_cartpole,
     "gym.CartPole-v1": _make_cartpole,   # the id of the reference GPU path's configurations/es_gym_config.json
     "Pendulum-v1": _make_pendulum,
+    "Acrobot-v1": _make_acrobot,
+    "gym.Acrobot-v1": _make_acrobot,
+    "MountainCar-v0": _make_mountaincar,         # MountainCarContinuous-v0 does not match this prefix
+    "gym.MountainCar-v0": _make_mountaincar,
 }

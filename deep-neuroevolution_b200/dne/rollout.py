@@ -253,7 +253,7 @@ class RolloutRunner:
 
 class EpisodeKernelRunner:
     """``RolloutRunner`` for environments whose episodes run entirely on the device (``env.device_episodes``:
-    ``dne.envs.CartPoleEnv``, ``dne.envs.PendulumEnv``): every member of every unit plays its whole episode inside ONE
+    ``dne.envs.CartPoleEnv``, ``AcrobotEnv``, ``MountainCarEnv``, ``PendulumEnv``): every member of every unit plays its whole episode inside ONE
     launch (``env.launch_episodes``), followed by one host sync for the results.  Same ``run`` signature and
     ``RolloutResult`` as ``RolloutRunner``.
 

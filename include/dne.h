@@ -184,6 +184,23 @@ int dne_cartpole_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_
                           int n_members, const double* d_init_state, int max_steps,
                           float* d_returns, int32_t* d_lengths, double* d_final_state, void* stream);
 
+/* gym's discrete-action classic_control tasks, whole episodes on the device (DESIGN.md 3.5) */
+#define DNE_EPISODE_CARTPOLE    0      /* CartPole-v1:    state (x, x_dot, theta, theta_dot), ob_dim 4, 2 actions, 500 steps */
+#define DNE_EPISODE_ACROBOT     1      /* Acrobot-v1:     state (theta1, theta2, dtheta1, dtheta2), ob_dim 6, 3 actions, 500 */
+#define DNE_EPISODE_MOUNTAINCAR 2      /* MountainCar-v0: state (position, velocity), ob_dim 2, 3 actions, 200 */
+
+/* dne_cartpole_episodes for any DNE_EPISODE_* task `env`: the same arguments, with d_init_state / d_final_state
+ * double[n][state_dim] (4, 4, 2) and 1 <= max_steps <= the task's TimeLimit (else DNE_ERR_ARG).  Observation: float32 of
+ * the task's observation vector; action: the first NaN logit if any, otherwise the first maximum; d_returns: the float64
+ * rewards (+1 per CartPole step; -1 per Acrobot step, 0 on the terminating one; -1 per MountainCar step) summed in step
+ * order and rounded to float32 once.  Supported nets: 1..4 dense layers of width <= 32, DNE_OB_VECTOR with the task's
+ * ob_dim, n_out = its action count, ReLU hidden layers, linear head, no batch norm; anything else returns DNE_ERR_UNSUP
+ * with the reason in dne_last_error(). */
+int dne_discrete_episodes(dne_ctx* ctx, int env, const dne_net_desc* net, const float* d_theta,
+                          const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                          int n_members, const double* d_init_state, int max_steps,
+                          float* d_returns, int32_t* d_lengths, double* d_final_state, void* stream);
+
 /* Pendulum-v1 (gymnasium classic_control pendulum.py, DESIGN.md 3.6) episodes run entirely on the device, one per member,
  * for MujocoPolicy 'continuous:' nets.  Weights as dne_cartpole_episodes; initial state d_init_state[m] = (th, thdot)
  * (float64); exactly max_steps (1..200) steps, there is no termination.  Per step: observation float32(cos th, sin th,

@@ -1,6 +1,7 @@
-"""CartPole-v1 throughput of the fused episode kernel at the es_gym_config population (needs an H100).
+"""CartPole-v1 (or Acrobot-v1 / MountainCar-v0) throughput of the fused episode kernel at the es_gym_config population
+(needs an H100).
 
-    python tools/cartpole_throughput.py [--gens 45] [--launches 50] [--out FILE.json]
+    python tools/cartpole_throughput.py [--env CartPole-v1] [--gens 45] [--launches 50] [--out FILE.json]
 
 Population: 5000 episodes per generation = 2500 antithetic pairs plus the 1 % evaluation share (eval_prob 0.01 of the
 2500 pairs: 25 episodes, run as 13 noiseless pairs), SimpleClassifier, noise_stdev 0.02, the 500-step limit.
@@ -10,6 +11,9 @@ Reports, from one process:
     --gens generations of configurations/cartpole_es.json (longer episodes);
   * the generation wall-clock of es_distributed.es.run_master on that configuration (median over generations 2..gens);
   * the card's name and power limit, read in the same run.
+--env Acrobot-v1 / MountainCar-v0 runs the same population of SimpleClassifier members (3 actions) through
+dne_discrete_episodes at the task's time limit, the trained weights coming from --gens generations of
+configurations/acrobot_es.json (ES) / mountaincar_ga.json (GA, the elite's weights).
 """
 import argparse
 import ctypes as C
@@ -26,11 +30,16 @@ import torch         # noqa: E402
 
 from dne import _ffi as F                        # noqa: E402
 from dne import nets                             # noqa: E402
-from dne.envs import CartPoleEnv                 # noqa: E402
+from dne.envs import AcrobotEnv, CartPoleEnv, MountainCarEnv   # noqa: E402
 from es_distributed import es as ES              # noqa: E402
+from es_distributed import ga as GA              # noqa: E402
 from es_distributed import policies              # noqa: E402
 
-CONFIG = os.path.join(ROOT, "deep-neuroevolution_b200", "configurations", "cartpole_es.json")
+CONFIGS = os.path.join(ROOT, "deep-neuroevolution_b200", "configurations")
+# env id -> (environment, DNE_EPISODE_* id, configuration, ob_dim, actions)
+TASKS = {"CartPole-v1": (CartPoleEnv, F.EPISODE_CARTPOLE, "cartpole_es.json", 4, 2),
+         "Acrobot-v1": (AcrobotEnv, F.EPISODE_ACROBOT, "acrobot_es.json", 6, 3),
+         "MountainCar-v0": (MountainCarEnv, F.EPISODE_MOUNTAINCAR, "mountaincar_ga.json", 2, 3)}
 
 
 def card():
@@ -39,8 +48,10 @@ def card():
     return {"name": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip() or q.stderr.strip()}
 
 
-def time_kernel(ctx, net, theta, n_pairs, n_eval_pairs, launches, seed=0):
-    """CUDA-event time of `launches` dne_cartpole_episodes launches over one generation's members."""
+def time_kernel(ctx, net, theta, n_pairs, n_eval_pairs, launches, seed=0, env_id="CartPole-v1"):
+    """CUDA-event time of `launches` dne_cartpole_episodes (dne_discrete_episodes for the other tasks) launches over one
+    generation's members."""
+    env_cls, episode_env = TASKS[env_id][:2]
     dev = torch.device("cuda", 0)
     rs = np.random.RandomState(seed)
     P = net.num_params
@@ -48,7 +59,8 @@ def time_kernel(ctx, net, theta, n_pairs, n_eval_pairs, launches, seed=0):
     pidx = rs.randint(0, ES.default_noise().count - P + 1, size=n_pairs)
     idx = np.concatenate([np.repeat(pidx, 2), np.zeros(2 * n_eval_pairs, np.int64)]).astype(np.int64)
     scale = np.concatenate([np.tile([0.02, -0.02], n_pairs), np.zeros(2 * n_eval_pairs)]).astype(np.float32)
-    init = CartPoleEnv(n, seed=seed).initial_states(n)
+    init = env_cls(n, seed=seed).initial_states(n)
+    limit = env_cls(1).max_episode_steps
     th = theta.contiguous()
     d_idx, d_sc = torch.from_numpy(idx).to(dev), torch.from_numpy(scale).to(dev)
     d_init = torch.from_numpy(init).to(dev)
@@ -56,8 +68,13 @@ def time_kernel(ctx, net, theta, n_pairs, n_eval_pairs, launches, seed=0):
     d_len = torch.empty(n, dtype=torch.int32, device=dev)
 
     def launch():
-        F.check(F.lib().dne_cartpole_episodes(ctx.handle, C.byref(net.desc), F.ptr(th), F.ptr(d_idx), F.ptr(d_sc), None, n,
-                                              F.ptr(d_init), 500, F.ptr(d_ret), F.ptr(d_len), None, F.stream_ptr()))
+        if env_id == "CartPole-v1":
+            F.check(F.lib().dne_cartpole_episodes(ctx.handle, C.byref(net.desc), F.ptr(th), F.ptr(d_idx), F.ptr(d_sc), None,
+                                                  n, F.ptr(d_init), 500, F.ptr(d_ret), F.ptr(d_len), None, F.stream_ptr()))
+        else:
+            F.check(F.lib().dne_discrete_episodes(ctx.handle, episode_env, C.byref(net.desc), F.ptr(th), F.ptr(d_idx),
+                                                  F.ptr(d_sc), None, n, F.ptr(d_init), limit, F.ptr(d_ret), F.ptr(d_len),
+                                                  None, F.stream_ptr()))
     for _ in range(3):
         launch()
     torch.cuda.synchronize()
@@ -75,29 +92,43 @@ def time_kernel(ctx, net, theta, n_pairs, n_eval_pairs, launches, seed=0):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--env", choices=sorted(TASKS), default="CartPole-v1")
     ap.add_argument("--gens", type=int, default=45)
     ap.add_argument("--launches", type=int, default=50)
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
     out = {"card": card()}
-    with open(CONFIG) as f:
+    env_cls, _, config, ob_dim, n_act = TASKS[args.env]
+    if args.env != "CartPole-v1":
+        out["env"] = args.env
+    with open(os.path.join(CONFIGS, config)) as f:
         exp = json.load(f)
     exp["config"]["snapshot_freq"] = 0
-    cfg = exp["config"]
-    n_pairs = cfg["episodes_per_batch"] // 2
-    n_eval_pairs = -(-int(round(n_pairs * cfg["eval_prob"])) // 2)
+    # the es_gym_config population: 5000 episodes, a 1 % evaluation share
+    n_pairs = 5000 // 2
+    n_eval_pairs = -(-int(round(n_pairs * 0.01)) // 2)
     ctx = ES.default_context()
-    net = nets.make_net("SimpleClassifier", num_actions=2, ob_dim=4)
-    env = CartPoleEnv(8, seed=0)
+    net = nets.make_net("SimpleClassifier", num_actions=n_act, ob_dim=ob_dim)
+    env = env_cls(8, seed=0)
     pol = policies.SimpleClassifierPolicy(env.observation_space, env.action_space, seed=0)
-    out["kernel_initial_theta"] = time_kernel(ctx, net, pol.device_theta, n_pairs, n_eval_pairs, args.launches)
+    out["kernel_initial_theta"] = time_kernel(ctx, net, pol.device_theta, n_pairs, n_eval_pairs, args.launches,
+                                              env_id=args.env)
 
     gens = []
-    theta = ES.run_master(None, None, exp, max_iterations=args.gens, env=env, seed=0,
-                          on_iteration=lambda it, st, ex: gens.append((st["TimeElapsedThisIter"], st["EpLenMean"],
-                                                                       st["EpisodesThisIter"], st["EvalEpCount"])))
-    out["kernel_trained_theta"] = time_kernel(ctx, net, torch.from_numpy(theta).cuda(), n_pairs, n_eval_pairs, args.launches)
+
+    def on_it(it, st, ex):
+        gens.append((st["TimeElapsedThisIter"], st.get("EpLenMean", 0.0), st.get("EpisodesThisIter", 0),
+                     st.get("EvalEpCount", 0)))
+        if "elite_theta" in ex:
+            out["_elite"] = ex["elite_theta"].clone()
+    if "population_size" in exp:                                   # the GA configuration
+        GA.run_master(None, None, exp, max_iterations=args.gens, env=env, seed=0, on_iteration=on_it)
+        theta = out.pop("_elite")
+    else:
+        theta = ES.run_master(None, None, exp, max_iterations=args.gens, env=env, seed=0, on_iteration=on_it)
+    theta = theta if torch.is_tensor(theta) else torch.from_numpy(theta).cuda()
+    out["kernel_trained_theta"] = time_kernel(ctx, net, theta, n_pairs, n_eval_pairs, args.launches, env_id=args.env)
     out["generations"] = [{"seconds": g[0], "ep_len_mean": g[1], "episodes": g[2], "eval_episodes": g[3]} for g in gens]
     out["generation_wallclock_s_median"] = float(np.median([g[0] for g in gens[1:]])) if len(gens) > 1 else gens[0][0]
     out["generation_wallclock_s_last"] = gens[-1][0]

@@ -168,6 +168,11 @@ knn_dist_kernel(const uint8_t* __restrict__ bc, const int32_t* __restrict__ bc_l
 }
 
 // mean of the k smallest distances per query (nses.py:28-32); k successive min-extractions, one CTA per query.
+// Order of numpy's sort: numbers ascending, NaN after every number (a NaN BC coordinate gives NaN distances), so a NaN is
+// taken only when no number is left and the mean is then NaN.  Taken entries are marked -1.0 (distances are never < 0).
+__device__ __forceinline__ bool dist_before(double a, double b) { return (a < b) || ((b != b) && (a == a)); }
+__device__ __forceinline__ bool dist_same(double a, double b) { return (a == b) || ((a != a) && (b != b)); }
+
 __global__ void __launch_bounds__(KNN_THREADS)
 knn_select_kernel(double* __restrict__ dist, int A, int k, float* __restrict__ novelty) {
     const int qi = blockIdx.x;
@@ -176,12 +181,12 @@ knn_select_kernel(double* __restrict__ dist, int A, int k, float* __restrict__ n
     __shared__ int si[KNN_THREADS];
     const int kk = min(k, A);
     double sum = 0.0;
-    for (int it = 0; it < kk; ++it) {
-        double bv = INFINITY;
+    for (int it = 0; it < kk; ++it) {         // A - it >= 1 entries are untaken: every iteration finds one
+        double bv = 0.0;
         int bi = -1;
         for (int j = threadIdx.x; j < A; j += KNN_THREADS) {
             const double v = d[j];
-            if (v >= 0.0 && (bi < 0 || v < bv)) { bv = v; bi = j; }
+            if (!(v < 0.0) && (bi < 0 || dist_before(v, bv))) { bv = v; bi = j; }
         }
         sv[threadIdx.x] = bv;
         si[threadIdx.x] = bi;
@@ -190,8 +195,9 @@ knn_select_kernel(double* __restrict__ dist, int A, int k, float* __restrict__ n
             if (threadIdx.x < o) {
                 const int oi = si[threadIdx.x + o];
                 const double ov = sv[threadIdx.x + o];
+                const double mv = sv[threadIdx.x];
                 const int mi = si[threadIdx.x];
-                if (oi >= 0 && (mi < 0 || ov < sv[threadIdx.x] || (ov == sv[threadIdx.x] && oi < mi))) {
+                if (oi >= 0 && (mi < 0 || dist_before(ov, mv) || (dist_same(ov, mv) && oi < mi))) {
                     sv[threadIdx.x] = ov;
                     si[threadIdx.x] = oi;
                 }
@@ -200,7 +206,7 @@ knn_select_kernel(double* __restrict__ dist, int A, int k, float* __restrict__ n
         }
         if (threadIdx.x == 0) {
             sum += sv[0];
-            d[si[0]] = -1.0;                                    // mark as taken (distances are >= 0)
+            d[si[0]] = -1.0;                                    // mark as taken
         }
         __syncthreads();
     }

@@ -302,7 +302,9 @@ int dne_knn_novelty(const uint8_t* d_bc, const int32_t* d_bc_len, int q,
                     int t_max, int D, int k, float* d_novelty, void* d_ws, size_t ws_bytes, void* stream);
 
 /* Same for vector BCs (MujocoPolicy: final (x, y) position / trajectory, policies.py:292-299): float64 [*, D] of equal
- * length, plain L2 distance in float64 (nses.py:12-20 with equal lengths), mean of the k smallest. */
+ * length, plain L2 distance in float64 (nses.py:12-20 with equal lengths), mean of the k smallest.  Distances are ordered
+ * like numpy's sort, NaN (from a NaN coordinate) after every number, so the novelty is NaN exactly when fewer than
+ * min(k, A) of the query's distances are numbers. */
 int dne_knn_novelty_vec(const double* d_bc, int q, const double* d_archive, int A, int D, int k, float* d_novelty,
                         void* d_ws, size_t ws_bytes, void* stream);
 

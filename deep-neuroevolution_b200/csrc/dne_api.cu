@@ -24,6 +24,10 @@ extern "C" int dne_abi_sizes(int* layer_desc_bytes, int* net_desc_bytes) {
     if (net_desc_bytes) *net_desc_bytes = (int)sizeof(dne_net_desc);
     return DNE_OK;
 }
+extern "C" int dne_abi_maze_size(int* maze_desc_bytes) {
+    if (maze_desc_bytes) *maze_desc_bytes = (int)sizeof(dne_maze_desc);
+    return DNE_OK;
+}
 
 extern "C" int dne_ctx_create(int device, dne_ctx** out) {
     DNE_CHECK_ARG(out, "out is null");
@@ -548,6 +552,51 @@ extern "C" int dne_pendulum_episodes(dne_ctx* ctx, const dne_net_desc* net, cons
                                                 (cudaStream_t)stream);
     if (rc) {
         dne_set_error("dne_pendulum_episodes: launch setup failed (%d)", rc);
+        return rc;
+    }
+    DNE_LAUNCH_CHECK();
+    return DNE_OK;
+}
+
+static int maze_net_check(const dne_net_desc* net, const char* fn) {
+    const char* why = "";
+    if (!dne_maze_net_supported(net, &why)) {
+        dne_set_error("%s: net not supported by the episode kernel: %s", fn, why);
+        return DNE_ERR_UNSUP;
+    }
+    return DNE_OK;
+}
+
+extern "C" int dne_maze_net_supported(const dne_net_desc* net) {
+    DNE_CHECK_ARG(net, "null net");
+    return maze_net_check(net, "dne_maze_net_supported");
+}
+
+extern "C" int dne_maze_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_desc* net, const float* d_theta,
+                                 const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                 int n_members, const double* d_init_state, int max_steps, const float* d_ob_mean,
+                                 const float* d_ob_std, const float* d_ac_noise, float* d_returns, float* d_signreturns,
+                                 int32_t* d_lengths, double* d_final_state, double* d_ob_sum, double* d_ob_sumsq,
+                                 void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    DNE_CHECK_ARG(maze, "null maze");
+    DNE_CHECK_ARG(maze->n_walls >= 0 && maze->n_walls <= DNE_MAZE_MAX_WALLS, "maze n_walls outside 0..64");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_signreturns && d_lengths,
+                  "null pointer");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1 && max_steps <= 400, "max_steps outside 1..400 (the maze's episode length)");
+    DNE_CHECK_ARG((d_ob_mean == nullptr) == (d_ob_std == nullptr), "pass both d_ob_mean and d_ob_std or neither");
+    DNE_CHECK_ARG((d_ob_sum == nullptr) == (d_ob_sumsq == nullptr), "pass both d_ob_sum and d_ob_sumsq or neither");
+    const int rc0 = maze_net_check(net, "dne_maze_episodes");
+    if (rc0) return rc0;
+    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
+    if (n_members == 0) return DNE_OK;
+    const int rc = dne_launch_maze_episodes(maze, net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx, n_members,
+                                            d_init_state, max_steps, d_ob_mean, d_ob_std, d_ac_noise, d_returns,
+                                            d_signreturns, d_lengths, d_final_state, d_ob_sum, d_ob_sumsq,
+                                            (cudaStream_t)stream);
+    if (rc) {
+        dne_set_error("dne_maze_episodes: launch setup failed (%d)", rc);
         return rc;
     }
     DNE_LAUNCH_CHECK();

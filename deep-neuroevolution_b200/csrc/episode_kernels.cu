@@ -1,17 +1,18 @@
 // episode_kernels.cu -- whole episodes of a device-resident environment in one launch.
 //
-// CartPole-v1, Acrobot-v1, MountainCar-v0 and Pendulum-v1 (gym classic_control): the policy has a few hundred to a few
-// tens of thousands of parameters and the environment step is a few dozen to a few hundred flops, so the per-tick runner
-// (one forward launch + a device -> host -> device round trip per step) would spend nearly all its time on overhead.  Here a
-// group of threads runs one member's episode from reset to the end: it builds the member's weights once in shared memory,
-// then loops observation -> dense forward -> action -> environment step on the device.
+// CartPole-v1, Acrobot-v1, MountainCar-v0, Pendulum-v1 (gym classic_control) and the hard maze: the policy has a few
+// hundred to a few tens of thousands of parameters and the environment step is a few dozen to a few hundred flops, so the
+// per-tick runner (one forward launch + a device -> host -> device round trip per step) would spend nearly all its time on
+// overhead.  Here a group of threads runs one member's episode from reset to the end: it builds the member's weights once
+// in shared memory, then loops observation -> dense forward -> action -> environment step on the device.
 //
-// Numerics contract (DESIGN.md 3.5, 3.6):
+// Numerics contract (DESIGN.md 3.5, 3.6, 3.7):
 //   * weights w = fl(theta[row] + fl(scale * noise[idx + j])) -- the same rounding as every other forward of the engine;
 //   * dense layers in fp32: each output a sequential fmaf over its inputs in index order, then + bias; the hidden layers'
 //     activation is apply_act (common.cuh), the head is linear;
 //   * the environment step in float64, in gym's operation order, every operation an explicit round-to-nearest intrinsic so
-//     nvcc cannot contract it into FMAs; sin / cos are CUDA's double sin / cos.
+//     nvcc cannot contract it into FMAs; sin / cos are CUDA's double sin / cos.  The maze steps in the reference's float32
+//     and double operations, explicit intrinsics too.
 // No workspace, no atomics, no device RNG: reruns are bit-identical.
 #include "common.cuh"
 #include "forward.cuh"
@@ -418,40 +419,282 @@ int dne_launch_discrete_episodes(int env, const dne_net_desc* net, const float* 
     }
 }
 
-// ---- Pendulum-v1 ------------------------------------------------------------------------------------------------------
-// gymnasium classic_control pendulum.py: g = 10, m = l = 1, dt = 0.05, max_speed = 8, max_torque = 2, TimeLimit 200, no
-// termination.  One member per group of min(max layer width, 256) threads, rounded up to a warp (thread t owns outputs
-// t, t + threads, ... of every layer); as many groups per CTA as maximise the members resident per SM, each group
-// synchronised by its own named barrier.  Thread 0 of a group keeps the float64 state, writes the normalised observation,
-// computes the head (n_out 1) and steps the pendulum.
-constexpr int PEND_OB_DIM = 3, PEND_ACTIONS = 1, PEND_MAX_STEPS = 200;
-constexpr int PEND_CTA_THREADS = 256;
-constexpr int PEND_MAX_GROUPS = 15;                   // named barriers 1..15 (0 is __syncthreads')
-constexpr size_t PEND_SMEM_LIMIT = 227 * 1024;        // H100 opt-in shared memory per CTA
+// ---- continuous-action tasks: Pendulum-v1, the hard maze ---------------------------------------------------------------
+// MujocoPolicy 'continuous:' nets.  One member per group of min(max layer width, 256) threads, rounded up to a warp
+// (thread t owns outputs t, t + threads, ... of every layer); as many groups per CTA as maximise the members resident per
+// SM, each group synchronised by its own named barrier.  The first Task::STEP_THREADS threads of a group (1, or the
+// group's first warp) keep the task's state and compute its observation; thread 0 writes the normalised observation,
+// keeps the observation sums, computes the linear head and adds the action noise; the same threads then step the task.
+// A task type supplies OB_DIM, N_OUT, STATE_DIM, TIME_LIMIT, STEP_THREADS, its Params (passed by value to the kernel),
+// load / store of the float64 state, ob(o, params, lane) (the full float32 observation in every stepping thread) and
+// step(a, params, lane) (returns the float32 reward).
+constexpr int CONT_CTA_THREADS = 256;
+constexpr int CONT_MAX_GROUPS = 15;                   // named barriers 1..15 (0 is __syncthreads')
+constexpr size_t CONT_SMEM_LIMIT = 227 * 1024;        // H100 opt-in shared memory per CTA
 
-struct PendulumGeom {
+struct NoParams {};
+
+// Pendulum-v1: gymnasium classic_control pendulum.py, g = 10, m = l = 1, dt = 0.05, max_speed = 8, max_torque = 2,
+// TimeLimit 200, no termination.
+struct PendulumTask {
+    static constexpr int OB_DIM = 3, N_OUT = 1, STATE_DIM = 2, TIME_LIMIT = 200, STEP_THREADS = 1;
+    static constexpr const char* OB_WHY = "Pendulum observations have ob_dim 3";
+    static constexpr const char* OUT_WHY = "Pendulum has one continuous action (n_out 1)";
+    using Params = NoParams;
+    double th = 0.0, thdot = 0.0;
+
+    __device__ __forceinline__ void load(const double* s) {
+        th = s[0];
+        thdot = s[1];
+    }
+    __device__ __forceinline__ void store(double* s) const {
+        s[0] = th;
+        s[1] = thdot;
+    }
+    __device__ __forceinline__ void ob(float* o, const Params&, int) const {      // float32([cos th, sin th, thdot])
+        o[0] = __double2float_rn(cos(th));
+        o[1] = __double2float_rn(sin(th));
+        o[2] = __double2float_rn(thdot);
+    }
+    // one step with the float32 action a[0] (already noised); the float64 reward rounded to float32, as BatchEnv.step
+    // returns it
+    __device__ __forceinline__ float step(const float* a, const Params&, int) {
+        return __double2float_rn(pendulum_step(th, thdot, a[0]));
+    }
+
+    // numpy's float64 divmod remainder (npy_divmod): fmod, then moved to the divisor's sign
+    static __device__ __forceinline__ double py_mod(double a, double b) {
+        double r = fmod(a, b);
+        if (r != 0.0) {
+            if ((r < 0.0) != (b < 0.0)) r = __dadd_rn(r, b);
+        } else {
+            r = copysign(0.0, b);
+        }
+        return r;
+    }
+    static __device__ __forceinline__ double pendulum_step(double& th, double& thdot, float a) {
+        const float u = a < -2.0f ? -2.0f : (a > 2.0f ? 2.0f : a);            // np.clip on the float32 action (NaN stays)
+        const double two_pi = __dmul_rn(2.0, CUDART_PI);
+        const double an = __dsub_rn(py_mod(__dadd_rn(th, CUDART_PI), two_pi), CUDART_PI);     // angle_normalize(th)
+        // costs = angle_normalize(th)**2 + 0.1 * thdot**2 + 0.001 * (u**2)   (u**2 is a float32 product)
+        const double costs = __dadd_rn(__dadd_rn(__dmul_rn(an, an), __dmul_rn(0.1, __dmul_rn(thdot, thdot))),
+                                       __dmul_rn(0.001, (double)__fmul_rn(u, u)));
+        // newthdot = thdot + (3 * g / (2 * l) * sin(th) + 3.0 / (m * l**2) * u) * dt, clipped to +-max_speed
+        double nthdot = __dadd_rn(thdot, __dmul_rn(__dadd_rn(__dmul_rn(15.0, sin(th)), __dmul_rn(3.0, (double)u)), 0.05));
+        nthdot = nthdot < -8.0 ? -8.0 : (nthdot > 8.0 ? 8.0 : nthdot);
+        th = __dadd_rn(th, __dmul_rn(nthdot, 0.05));
+        thdot = nthdot;
+        return -costs;
+    }
+};
+
+// The hard maze of the reference's GPU path (gym_tensorflow/maze/maze.h stepped as tf_maze.cpp's MazeEnvironment;
+// DESIGN.md 3.7).  A navigator of radius 8 with 6 rangefinders (range 100) and a 4-sector goal radar; observation
+// [1, range_i / 100, radar_j]; actions (turn, speed) + 0.5 through interpret_outputs' rate limits and clamps; Update()
+// moves it unless the new position is within the radius of a wall; the only reward is -distance to the goal on the
+// 400th step.  Single-precision C++ restated operation by operation: every float operation an explicit __f*_rn
+// intrinsic (nvcc would contract products into FMAs), double where the C++ promotes, cosf / sinf / atanf where it calls
+// the float overloads, double cos / sin where it calls those.  The state is float32 values kept in float64.
+struct MazeParams {
+    float4 walls[DNE_MAZE_MAX_WALLS];                 // (ax, ay, bx, by)
+    int n_walls;
+    int sticky;                                       // the file's collision flag: a hit freezes the navigator
+    float gx, gy;                                     // goal
+    float ray_dx[6], ray_dy[6];                       // fl(cosf(rad_i) * 100), fl(sinf(rad_i) * 100), host libm
+};
+
+__device__ __forceinline__ float maze_deg2rad(float deg) {   // angle/180.0*3.1415926 in double, stored to float
+    return __double2float_rn(__dmul_rn(__ddiv_rn((double)deg, 180.0), 3.1415926));
+}
+
+__device__ __forceinline__ float maze_dist(float ax, float ay, float bx, float by) {   // Point(a).distance(b)
+    const float dx = __fsub_rn(bx, ax), dy = __fsub_rn(by, ay);
+    return __fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));
+}
+
+struct MazeTask {
+    static constexpr int OB_DIM = 11, N_OUT = 2, STATE_DIM = 7, TIME_LIMIT = 400, STEP_THREADS = 32;
+    static constexpr const char* OB_WHY = "maze observations have ob_dim 11";
+    static constexpr const char* OUT_WHY = "the maze has two continuous actions (n_out 2)";
+    using Params = MazeParams;
+    float x = 0.f, y = 0.f, heading = 0.f, speed = 0.f, ang_vel = 0.f;
+    int t = 0;
+    bool collide = false;
+
+    __device__ __forceinline__ void load(const double* s) {
+        x = (float)s[0];
+        y = (float)s[1];
+        heading = (float)s[2];
+        speed = (float)s[3];
+        ang_vel = (float)s[4];
+        t = (int)s[5];
+        collide = s[6] != 0.0;
+    }
+    __device__ __forceinline__ void store(double* s) const {
+        s[0] = x;
+        s[1] = y;
+        s[2] = heading;
+        s[3] = speed;
+        s[4] = ang_vel;
+        s[5] = t;
+        s[6] = collide ? 1.0 : 0.0;
+    }
+
+    // Rangefinders: the 6 x n_walls ray-wall tests are dealt over the warp; each lane keeps a running minimum per ray
+    // starting from the range 100, and the lanes' minima are combined with the same comparison.  The reference's
+    // sequential `if (found < range) range = found` keeps the minimum of the numbers found (a NaN never compares less),
+    // and a minimum under `<` is the same in any order, so the result is exact.
+    __device__ __forceinline__ void ob(float* o, const Params& p, int lane) const {
+        const float rh = maze_deg2rad(heading);
+        const float c = cosf(rh), sn = sinf(rh);
+        float rng[6];
+#pragma unroll
+        for (int i = 0; i < 6; ++i) rng[i] = 100.0f;
+        for (int k = lane; k < 6 * p.n_walls; k += 32) {
+            const int ray = k / p.n_walls;
+            const float4 w = p.walls[k - ray * p.n_walls];
+            // the projected point (x + cos(rad)*100, y + sin(rad)*100) rotated by the heading about (x, y)
+            const float ox = __fsub_rn(__fadd_rn(x, p.ray_dx[ray]), x), oy = __fsub_rn(__fadd_rn(y, p.ray_dy[ray]), y);
+            const float px = __fadd_rn(__fsub_rn(__fmul_rn(c, ox), __fmul_rn(sn, oy)), x);
+            const float py = __fadd_rn(__fadd_rn(__fmul_rn(sn, ox), __fmul_rn(c, oy)), y);
+            // Line::intersection of the wall (A, B) with (x, y) -> (px, py); rBot and sBot are the same expression
+            const float ay_c = __fsub_rn(w.y, y), ax_c = __fsub_rn(w.x, x), bax = __fsub_rn(w.z, w.x),
+                        bay = __fsub_rn(w.w, w.y), dxc = __fsub_rn(px, x), dyc = __fsub_rn(py, y);
+            const float rtop = __fsub_rn(__fmul_rn(ay_c, dxc), __fmul_rn(ax_c, dyc));
+            const float rbot = __fsub_rn(__fmul_rn(bax, dyc), __fmul_rn(bay, dxc));
+            const float stop = __fsub_rn(__fmul_rn(ay_c, bax), __fmul_rn(ax_c, bay));
+            if (rbot == 0.0f) continue;
+            const float r = __fdiv_rn(rtop, rbot), s = __fdiv_rn(stop, rbot);
+            if (!(r > 0.0f && r < 1.0f && s > 0.0f && s < 1.0f)) continue;
+            const float d = maze_dist(__fadd_rn(w.x, __fmul_rn(r, bax)), __fadd_rn(w.y, __fmul_rn(r, bay)), x, y);
+#pragma unroll
+            for (int i = 0; i < 6; ++i)
+                if (ray == i && d < rng[i]) rng[i] = d;
+        }
+#pragma unroll
+        for (int i = 0; i < 6; ++i) {
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) {
+                const float v = __shfl_xor_sync(0xffffffffu, rng[i], off);
+                if (v < rng[i]) rng[i] = v;
+            }
+        }
+        o[0] = 1.0f;
+#pragma unroll
+        for (int i = 0; i < 6; ++i) o[1 + i] = __fdiv_rn(rng[i], 100.0f);
+        // the goal radar: the goal rotated by -heading about (x, y), moved to the navigator's frame, Point::angle()
+        const float rg = maze_deg2rad(-heading);
+        const float cg = cosf(rg), sg = sinf(rg);
+        const float gx = __fsub_rn(p.gx, x), gy = __fsub_rn(p.gy, y);
+        const float tx = __fsub_rn(__fadd_rn(__fsub_rn(__fmul_rn(cg, gx), __fmul_rn(sg, gy)), x), x);
+        const float ty = __fsub_rn(__fadd_rn(__fadd_rn(__fmul_rn(sg, gx), __fmul_rn(cg, gy)), y), y);
+        float ang;
+        if (tx == 0.0f) {
+            ang = ty > 0.0f ? 90.0f : 270.0f;
+        } else {
+            ang = __double2float_rn(__dmul_rn(__ddiv_rn((double)atanf(__fdiv_rn(ty, tx)), 3.1415926), 180.0));
+            if (!(tx > 0.0f)) ang = __double2float_rn(__dadd_rn((double)ang, 180.0));
+        }
+        const double ang360 = __dadd_rn((double)ang, 360.0);
+        const float lo[4] = {315.0f, 45.0f, 135.0f, 225.0f}, hi[4] = {405.0f, 135.0f, 225.0f, 315.0f};
+#pragma unroll
+        for (int j = 0; j < 4; ++j)      // half-open sectors, tested on the angle and on the angle + 360 (in double)
+            o[7 + j] = ((ang >= lo[j] && ang < hi[j]) || (ang360 >= (double)lo[j] && ang360 < (double)hi[j])) ? 1.0f
+                                                                                                             : 0.0f;
+    }
+
+    // Line::distance(n) < radius for one wall
+    static __device__ __forceinline__ bool hits(const float4 w, float nx, float ny) {
+        const float bax = __fsub_rn(w.z, w.x), bay = __fsub_rn(w.w, w.y);
+        const float utop = __fadd_rn(__fmul_rn(__fsub_rn(nx, w.x), bax), __fmul_rn(__fsub_rn(ny, w.y), bay));
+        float ubot = maze_dist(w.x, w.y, w.z, w.w);
+        ubot = __fmul_rn(ubot, ubot);
+        float d;
+        if (ubot == 0.0f) {
+            d = 0.0f;
+        } else {
+            const float u = __fdiv_rn(utop, ubot);
+            if (u < 0.0f || u > 1.0f) {
+                const float d1 = maze_dist(w.x, w.y, nx, ny), d2 = maze_dist(w.z, w.w, nx, ny);
+                d = d1 < d2 ? d1 : d2;
+            } else {
+                d = maze_dist(__fadd_rn(w.x, __fmul_rn(u, bax)), __fadd_rn(w.y, __fmul_rn(u, bay)), nx, ny);
+            }
+        }
+        return d < 8.0f;
+    }
+
+    // interpret_outputs(float(a0) + 0.5, 0.5 + float(a1)), Update(), one more step taken; every lane of the warp steps
+    // the same state, the collision tests (any wall within the radius, an order-free OR) dealt over the lanes
+    __device__ __forceinline__ float step(const float* a, const Params& p, int lane) {
+        float o1 = __double2float_rn(__dadd_rn((double)a[0], 0.5)), o2 = __double2float_rn(__dadd_rn(0.5, (double)a[1]));
+        if (o1 > 1.0f) o1 = 1.0f;
+        if (o1 < 0.0f) o1 = 0.0f;
+        if (o2 > 1.0f) o2 = 1.0f;
+        if (o2 < 0.0f) o2 = 0.0f;
+        float d_ang = __fsub_rn(__double2float_rn(__dmul_rn(__dsub_rn((double)o1, 0.5), 6.0)), ang_vel);
+        float d_speed = __fsub_rn(__double2float_rn(__dmul_rn(__dsub_rn((double)o2, 0.5), 6.0)), speed);
+        if ((double)d_ang >= 0.2) d_ang = 0.2f;                   // float against double 0.2, assigned as float
+        if ((double)d_ang <= -0.2) d_ang = -0.2f;
+        if ((double)d_speed >= 0.2) d_speed = 0.2f;
+        if ((double)d_speed <= -0.2) d_speed = -0.2f;
+        ang_vel = __fadd_rn(ang_vel, d_ang);
+        speed = __fadd_rn(speed, d_speed);
+        if (speed > 3.0f) speed = 3.0f;
+        if (speed < -3.0f) speed = -3.0f;
+        if (ang_vel > 3.0f) ang_vel = 3.0f;
+        if (ang_vel < -3.0f) ang_vel = -3.0f;
+        // Update(): the velocity from the heading before the turn, in double
+        const double h = __dmul_rn(__ddiv_rn((double)heading, 180.0), 3.1415926);
+        const float vx = __double2float_rn(__dmul_rn(cos(h), (double)speed));
+        const float vy = __double2float_rn(__dmul_rn(sin(h), (double)speed));
+        heading = __fadd_rn(heading, ang_vel);
+        if (heading > 360.0f) heading = __fsub_rn(heading, 360.0f);
+        if (heading < 0.0f) heading = __fadd_rn(heading, 360.0f);
+        const float nx = __fadd_rn(vx, x), ny = __fadd_rn(vy, y);
+        bool hit = false;
+        if (!collide) {
+            for (int j = lane; j < p.n_walls; j += 32) hit = hit || hits(p.walls[j], nx, ny);
+            hit = __any_sync(0xffffffffu, hit);
+        }
+        if (!collide && !hit) {
+            x = nx;
+            y = ny;
+        } else if (p.sticky) {
+            collide = true;
+        }
+        t += 1;
+        if (t < TIME_LIMIT) return 0.0f;
+        float d = maze_dist(x, y, p.gx, p.gy);                    // distance_to_target(): a NaN distance counts 500
+        if (d != d) d = 500.0f;
+        return -d;
+    }
+};
+
+struct ContinuousGeom {
     int threads;                                      // threads per member: min(max layer width, 256), a multiple of 32
     int act_pad;                                      // floats of one activation buffer: max layer width rounded up to 32
     size_t member_bytes;                              // weights + two activation buffers
 };
 
-static PendulumGeom pendulum_geom(const dne_net_desc* net) {
-    int width = PEND_OB_DIM;
+template <class Task>
+static ContinuousGeom continuous_geom(const dne_net_desc* net) {
+    int width = Task::OB_DIM;
     for (int l = 0; l < net->n_layers; ++l) width = width > net->layers[l].cout ? width : net->layers[l].cout;
-    PendulumGeom g;
+    ContinuousGeom g;
     g.act_pad = (width + 31) / 32 * 32;
-    g.threads = g.act_pad < PEND_CTA_THREADS ? g.act_pad : PEND_CTA_THREADS;
+    g.threads = g.act_pad < CONT_CTA_THREADS ? g.act_pad : CONT_CTA_THREADS;
     g.member_bytes = ((size_t)(net->num_params + 31) / 32 * 32 + 2 * (size_t)g.act_pad) * sizeof(float);
     return g;
 }
 
-// Which nets the fused Pendulum kernel runs: 1..DNE_MAX_LAYERS dense layers, vector observations of dimension 3, 1
-// output, tanh or ReLU hidden layers, a linear head, no batch norm, and one member's weights plus its two activation
-// buffers within one CTA's shared memory (hidden [200, 200] fits, [256, 256] does not).  Any layer width runs: a group
-// has at most 256 threads, each looping over its outputs.
-bool dne_pendulum_net_supported(const dne_net_desc* net, const char** why) {
-    if (!episode_net_common(net, DNE_MAX_LAYERS, PEND_OB_DIM, PEND_ACTIONS, "Pendulum observations have ob_dim 3",
-                            "Pendulum has one continuous action (n_out 1)", why))
+// Which nets the continuous episode kernel runs for Task: 1..DNE_MAX_LAYERS dense layers, vector observations of
+// dimension Task::OB_DIM, Task::N_OUT outputs, tanh or ReLU hidden layers, a linear head, no batch norm, and one member's
+// weights plus its two activation buffers within one CTA's shared memory (for Pendulum hidden [200, 200] fits,
+// [256, 256] does not).  Any layer width runs: a group has at most 256 threads, each looping over its outputs.
+template <class Task>
+static bool continuous_net_supported(const dne_net_desc* net, const char** why) {
+    if (!episode_net_common(net, DNE_MAX_LAYERS, Task::OB_DIM, Task::N_OUT, Task::OB_WHY, Task::OUT_WHY, why))
         return false;
     for (int l = 0; l < net->n_layers; ++l) {
         const int act = net->layers[l].act;
@@ -460,54 +703,38 @@ bool dne_pendulum_net_supported(const dne_net_desc* net, const char** why) {
             return false;
         }
     }
-    if (net->num_params > (1 << 24) || pendulum_geom(net).member_bytes > PEND_SMEM_LIMIT) {
+    if (net->num_params > (1 << 24) || continuous_geom<Task>(net).member_bytes > CONT_SMEM_LIMIT) {
         *why = "one member's weights and activations exceed a CTA's shared memory (227 KB)";
         return false;
     }
     return true;
 }
 
+bool dne_pendulum_net_supported(const dne_net_desc* net, const char** why) {
+    return continuous_net_supported<PendulumTask>(net, why);
+}
+
+bool dne_maze_net_supported(const dne_net_desc* net, const char** why) {
+    return continuous_net_supported<MazeTask>(net, why);
+}
+
 __device__ __forceinline__ void group_sync(int id, int nthr) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthr) : "memory");
 }
 
-// numpy's float64 divmod remainder (npy_divmod): fmod, then moved to the divisor's sign
-__device__ __forceinline__ double py_mod(double a, double b) {
-    double r = fmod(a, b);
-    if (r != 0.0) {
-        if ((r < 0.0) != (b < 0.0)) r = __dadd_rn(r, b);
-    } else {
-        r = copysign(0.0, b);
-    }
-    return r;
-}
-
-// One Pendulum-v1 step with the float32 action a (already noised): updates (th, thdot), returns the float64 reward.
-__device__ __forceinline__ double pendulum_step(double& th, double& thdot, float a) {
-    const float u = a < -2.0f ? -2.0f : (a > 2.0f ? 2.0f : a);            // np.clip on the float32 action (NaN stays)
-    const double two_pi = __dmul_rn(2.0, CUDART_PI);
-    const double an = __dsub_rn(py_mod(__dadd_rn(th, CUDART_PI), two_pi), CUDART_PI);     // angle_normalize(th)
-    // costs = angle_normalize(th)**2 + 0.1 * thdot**2 + 0.001 * (u**2)   (u**2 is a float32 product)
-    const double costs = __dadd_rn(__dadd_rn(__dmul_rn(an, an), __dmul_rn(0.1, __dmul_rn(thdot, thdot))),
-                                   __dmul_rn(0.001, (double)__fmul_rn(u, u)));
-    // newthdot = thdot + (3 * g / (2 * l) * sin(th) + 3.0 / (m * l**2) * u) * dt, clipped to +-max_speed
-    double nthdot = __dadd_rn(thdot, __dmul_rn(__dadd_rn(__dmul_rn(15.0, sin(th)), __dmul_rn(3.0, (double)u)), 0.05));
-    nthdot = nthdot < -8.0 ? -8.0 : (nthdot > 8.0 ? 8.0 : nthdot);
-    th = __dadd_rn(th, __dmul_rn(nthdot, 0.05));
-    thdot = nthdot;
-    return -costs;
-}
-
-// No spills (40-byte stack frame: double sin / cos's slow-path argument reduction; registers in DESIGN.md 3.6).  Shared
-// memory bounds the residency: hidden [64, 64] keeps 12 members (24 warps) per SM, [128, 128] 3, [200, 200] 1.
-__global__ void __launch_bounds__(PEND_CTA_THREADS)
-pendulum_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, const float* __restrict__ theta,
-                        const float* __restrict__ noise, const int64_t* __restrict__ noise_idx,
-                        const float* __restrict__ scale, const int32_t* __restrict__ theta_idx, int n_members,
-                        const double* __restrict__ init_state, int max_steps, const float* __restrict__ ob_mean,
-                        const float* __restrict__ ob_std, const float* __restrict__ ac_noise, float* __restrict__ returns,
-                        float* __restrict__ signreturns, int32_t* __restrict__ lengths, double* __restrict__ final_state,
-                        double* __restrict__ ob_sum, double* __restrict__ ob_sumsq) {
+// No spills (registers in DESIGN.md 3.6, 3.7).  Shared memory bounds the residency: for Pendulum hidden [64, 64] keeps
+// 12 members (24 warps) per SM, [128, 128] 3, [200, 200] 1.
+template <class Task>
+__global__ void __launch_bounds__(CONT_CTA_THREADS)
+continuous_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, const __grid_constant__ typename Task::Params prm,
+                          const float* __restrict__ theta, const float* __restrict__ noise,
+                          const int64_t* __restrict__ noise_idx, const float* __restrict__ scale,
+                          const int32_t* __restrict__ theta_idx, int n_members, const double* __restrict__ init_state,
+                          int max_steps, const float* __restrict__ ob_mean, const float* __restrict__ ob_std,
+                          const float* __restrict__ ac_noise, float* __restrict__ returns, float* __restrict__ signreturns,
+                          int32_t* __restrict__ lengths, double* __restrict__ final_state, double* __restrict__ ob_sum,
+                          double* __restrict__ ob_sumsq) {
+    constexpr int OB = Task::OB_DIM, NO = Task::N_OUT;
     extern __shared__ float ep_smem[];
     const int grp = threadIdx.x / threads, t = threadIdx.x - grp * threads;
     if (grp >= groups) return;
@@ -520,33 +747,28 @@ pendulum_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, co
 
     build_member_weights(w, net, theta, noise, noise_idx, scale, theta_idx, m, t, threads);
 
-    double th = 0.0, thdot = 0.0, ret = 0.0, sret = 0.0;
-    double os0 = 0.0, os1 = 0.0, os2 = 0.0, oq0 = 0.0, oq1 = 0.0, oq2 = 0.0;
-    if (t == 0) {
-        th = init_state[2 * m + 0];
-        thdot = init_state[2 * m + 1];
-    }
+    Task env;
+    double ret = 0.0, sret = 0.0;
+    double os[OB], oq[OB];
+#pragma unroll
+    for (int k = 0; k < OB; ++k) os[k] = oq[k] = 0.0;
+    if (t < Task::STEP_THREADS) env.load(init_state + (int64_t)Task::STATE_DIM * m);
     const int L = net.n_layers;
     for (int step = 0; step < max_steps; ++step) {
-        if (t == 0) {                         // observation float32([cos th, sin th, thdot]), normalised as ob_norm_kernel
-            const float o0 = __double2float_rn(cos(th)), o1 = __double2float_rn(sin(th)), o2 = __double2float_rn(thdot);
-            if (ob_sum) {                     // ob_stat_accum_kernel's sums of the unnormalised observation
-                os0 = __dadd_rn(os0, (double)o0);
-                os1 = __dadd_rn(os1, (double)o1);
-                os2 = __dadd_rn(os2, (double)o2);
-                oq0 = __dadd_rn(oq0, __dmul_rn((double)o0, (double)o0));
-                oq1 = __dadd_rn(oq1, __dmul_rn((double)o1, (double)o1));
-                oq2 = __dadd_rn(oq2, __dmul_rn((double)o2, (double)o2));
+        if (t < Task::STEP_THREADS) {         // the observation, normalised as ob_norm_kernel
+            float o[OB];
+            env.ob(o, prm, t);
+            if (t == 0) {
+#pragma unroll
+                for (int k = 0; k < OB; ++k) {
+                    if (ob_sum) {             // ob_stat_accum_kernel's sums of the unnormalised observation
+                        os[k] = __dadd_rn(os[k], (double)o[k]);
+                        oq[k] = __dadd_rn(oq[k], __dmul_rn((double)o[k], (double)o[k]));
+                    }
+                    buf0[k] = ob_mean ? fminf(fmaxf(__fdiv_rn(__fsub_rn(o[k], ob_mean[k]), ob_std[k]), -5.0f), 5.0f)
+                                      : o[k];
+                }
             }
-            float x0 = o0, x1 = o1, x2 = o2;
-            if (ob_mean) {
-                x0 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x0, ob_mean[0]), ob_std[0]), -5.0f), 5.0f);
-                x1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x1, ob_mean[1]), ob_std[1]), -5.0f), 5.0f);
-                x2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x2, ob_mean[2]), ob_std[2]), -5.0f), 5.0f);
-            }
-            buf0[0] = x0;
-            buf0[1] = x1;
-            buf0[2] = x2;
         }
         group_sync(bar, threads);
         // hidden layers: all threads, ping-pong buffers, one barrier per layer (a layer's reads of its output buffer, by
@@ -568,57 +790,66 @@ pendulum_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, co
             y = (float*)x;
             x = nx;
         }
-        if (t == 0) {                         // the linear head (n_out 1), the action noise, the environment step
-            const int K = net.cin[L - 1];
-            const float* wl = w + net.off_w[L - 1];
-            float acc = 0.0f;
+        if (t < Task::STEP_THREADS) {         // the linear head, the action noise, the environment step
+            float a[NO];
+            if (t == 0) {
+                const int K = net.cin[L - 1];
+                const float* wl = w + net.off_w[L - 1];
+#pragma unroll
+                for (int j = 0; j < NO; ++j) {
+                    float acc = 0.0f;
 #pragma unroll 4
-            for (int k = 0; k < K; ++k) acc = fmaf(x[k], wl[k], acc);
-            if (net.off_b[L - 1] >= 0) acc = __fadd_rn(acc, w[net.off_b[L - 1]]);
-            const float a = ac_noise ? __fadd_rn(acc, ac_noise[(int64_t)m * max_steps + step]) : acc;
-            const float r = __double2float_rn(pendulum_step(th, thdot, a));       // BatchEnv.step returns float32
-            ret = __dadd_rn(ret, (double)r);
-            sret = __dadd_rn(sret, r > 0.0f ? 1.0 : r < 0.0f ? -1.0 : (double)r);    // np.sign (0 -> 0, NaN -> NaN)
+                    for (int k = 0; k < K; ++k) acc = fmaf(x[k], wl[k * NO + j], acc);
+                    if (net.off_b[L - 1] >= 0) acc = __fadd_rn(acc, w[net.off_b[L - 1] + j]);
+                    a[j] = ac_noise ? __fadd_rn(acc, ac_noise[((int64_t)m * max_steps + step) * NO + j]) : acc;
+                }
+            }
+            if (Task::STEP_THREADS > 1) {
+#pragma unroll
+                for (int j = 0; j < NO; ++j) a[j] = __shfl_sync(0xffffffffu, a[j], 0);
+            }
+            const float r = env.step(a, prm, t);
+            if (t == 0) {
+                ret = __dadd_rn(ret, (double)r);
+                sret = __dadd_rn(sret, r > 0.0f ? 1.0 : r < 0.0f ? -1.0 : (double)r);    // np.sign (0 -> 0, NaN -> NaN)
+            }
         }
     }
     if (t == 0) {
         returns[m] = __double2float_rn(ret);
         signreturns[m] = __double2float_rn(sret);
         lengths[m] = max_steps;
-        if (final_state) {
-            final_state[2 * m + 0] = th;
-            final_state[2 * m + 1] = thdot;
-        }
+        if (final_state) env.store(final_state + (int64_t)Task::STATE_DIM * m);
         if (ob_sum) {
-            ob_sum[3 * m + 0] = os0;
-            ob_sum[3 * m + 1] = os1;
-            ob_sum[3 * m + 2] = os2;
-            ob_sumsq[3 * m + 0] = oq0;
-            ob_sumsq[3 * m + 1] = oq1;
-            ob_sumsq[3 * m + 2] = oq2;
+#pragma unroll
+            for (int k = 0; k < OB; ++k) {
+                ob_sum[(int64_t)OB * m + k] = os[k];
+                ob_sumsq[(int64_t)OB * m + k] = oq[k];
+            }
         }
     }
 }
 
-int dne_launch_pendulum_episodes(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,
-                                 const float* scale, const int32_t* theta_idx, int n_members, const double* init_state,
-                                 int max_steps, const float* ob_mean, const float* ob_std, const float* ac_noise,
-                                 float* returns, float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
-                                 double* ob_sumsq, cudaStream_t st) {
+template <class Task>
+static int launch_continuous(const dne_net_desc* net, const typename Task::Params& prm, const float* theta,
+                             const float* noise, const int64_t* noise_idx, const float* scale, const int32_t* theta_idx,
+                             int n_members, const double* init_state, int max_steps, const float* ob_mean,
+                             const float* ob_std, const float* ac_noise, float* returns, float* signreturns,
+                             int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st) {
     const EpisodeNet en = make_episode_net(net);
-    const PendulumGeom g = pendulum_geom(net);
-    if (cudaFuncSetAttribute(pendulum_episode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PEND_SMEM_LIMIT) !=
-        cudaSuccess)
+    const ContinuousGeom g = continuous_geom<Task>(net);
+    auto kern = continuous_episode_kernel<Task>;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CONT_SMEM_LIMIT) != cudaSuccess)
         return DNE_ERR_CUDA;
     // members per CTA: the count that keeps the most members resident per SM (registers, shared memory, threads, as the
-    // occupancy calculator counts them); on a tie the more (hidden [64, 64], 5000 members on an H100: 4 per CTA 2.74 and
-    // 2.84 ms in two runs, 2 per CTA 3.05 ms, both with 12 members resident per SM)
+    // occupancy calculator counts them); on a tie the more (Pendulum hidden [64, 64], 5000 members on an H100: 4 per CTA
+    // 2.74 and 2.84 ms in two runs, 2 per CTA 3.05 ms, both with 12 members resident per SM)
     int groups = 1, best = 0;
-    const int max_groups = PEND_CTA_THREADS / g.threads < PEND_MAX_GROUPS ? PEND_CTA_THREADS / g.threads : PEND_MAX_GROUPS;
-    for (int gr = 1; gr <= max_groups && (size_t)gr * g.member_bytes <= PEND_SMEM_LIMIT; ++gr) {
+    const int max_groups = CONT_CTA_THREADS / g.threads < CONT_MAX_GROUPS ? CONT_CTA_THREADS / g.threads : CONT_MAX_GROUPS;
+    for (int gr = 1; gr <= max_groups && (size_t)gr * g.member_bytes <= CONT_SMEM_LIMIT; ++gr) {
         int blocks = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, pendulum_episode_kernel, gr * g.threads,
-                                                          (size_t)gr * g.member_bytes) != cudaSuccess)
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, gr * g.threads, (size_t)gr * g.member_bytes) !=
+            cudaSuccess)
             return DNE_ERR_CUDA;
         if (blocks * gr >= best) {
             best = blocks * gr;
@@ -627,9 +858,44 @@ int dne_launch_pendulum_episodes(const dne_net_desc* net, const float* theta, co
     }
     const size_t smem = (size_t)groups * g.member_bytes;
     const unsigned grid = (unsigned)((n_members + groups - 1) / groups);
-    pendulum_episode_kernel<<<grid, groups * g.threads, smem, st>>>(
-        en, g.threads, g.act_pad, groups, theta, noise, noise_idx, scale, theta_idx, n_members, init_state, max_steps,
-        ob_mean, ob_std, ac_noise, returns, signreturns, lengths, final_state, ob_sum, ob_sumsq);
+    kern<<<grid, groups * g.threads, smem, st>>>(en, g.threads, g.act_pad, groups, prm, theta, noise, noise_idx, scale,
+                                                 theta_idx, n_members, init_state, max_steps, ob_mean, ob_std, ac_noise,
+                                                 returns, signreturns, lengths, final_state, ob_sum, ob_sumsq);
     DNE_LAUNCHED(1);
     return DNE_OK;
+}
+
+int dne_launch_pendulum_episodes(const dne_net_desc* net, const float* theta, const float* noise, const int64_t* noise_idx,
+                                 const float* scale, const int32_t* theta_idx, int n_members, const double* init_state,
+                                 int max_steps, const float* ob_mean, const float* ob_std, const float* ac_noise,
+                                 float* returns, float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
+                                 double* ob_sumsq, cudaStream_t st) {
+    return launch_continuous<PendulumTask>(net, NoParams{}, theta, noise, noise_idx, scale, theta_idx, n_members,
+                                           init_state, max_steps, ob_mean, ob_std, ac_noise, returns, signreturns, lengths,
+                                           final_state, ob_sum, ob_sumsq, st);
+}
+
+int dne_launch_maze_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta, const float* noise,
+                             const int64_t* noise_idx, const float* scale, const int32_t* theta_idx, int n_members,
+                             const double* init_state, int max_steps, const float* ob_mean, const float* ob_std,
+                             const float* ac_noise, float* returns, float* signreturns, int32_t* lengths,
+                             double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st) {
+    MazeParams p = {};
+    p.n_walls = maze->n_walls;
+    p.sticky = maze->collisions_stick != 0;
+    p.gx = maze->goal[0];
+    p.gy = maze->goal[1];
+    for (int j = 0; j < maze->n_walls; ++j)
+        p.walls[j] = make_float4(maze->walls[j][0], maze->walls[j][1], maze->walls[j][2], maze->walls[j][3]);
+    // the rangefinders' own directions: constant arguments, so computed here with the host C library's cosf / sinf,
+    // which the reference calls too (float rad = angle/180.0*3.1415926; cos(rad)*range in float)
+    const float angles[6] = {-90.0f, -45.0f, 0.0f, 45.0f, 90.0f, -180.0f};
+    for (int i = 0; i < 6; ++i) {
+        volatile float rad = (float)((double)angles[i] / 180.0 * 3.1415926);   // volatile: no compile-time folding
+        p.ray_dx[i] = cosf(rad) * 100.0f;
+        p.ray_dy[i] = sinf(rad) * 100.0f;
+    }
+    return launch_continuous<MazeTask>(net, p, theta, noise, noise_idx, scale, theta_idx, n_members, init_state, max_steps,
+                                       ob_mean, ob_std, ac_noise, returns, signreturns, lengths, final_state, ob_sum,
+                                       ob_sumsq, st);
 }

@@ -109,6 +109,13 @@ int dne_launch_pendulum_episodes(const dne_net_desc* net, const float* theta, co
                                  int max_steps, const float* ob_mean, const float* ob_std, const float* ac_noise,
                                  float* returns, float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
                                  double* ob_sumsq, cudaStream_t st);
+// episode_kernels.cu: whole hard-maze episodes on the device (dne_maze_episodes); `maze` already checked
+bool dne_maze_net_supported(const dne_net_desc* net, const char** why);
+int dne_launch_maze_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta, const float* noise,
+                             const int64_t* noise_idx, const float* scale, const int32_t* theta_idx, int n_members,
+                             const double* init_state, int max_steps, const float* ob_mean, const float* ob_std,
+                             const float* ac_noise, float* returns, float* signreturns, int32_t* lengths,
+                             double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st);
 
 int dne_launch_theta_gemm_tc(const float* X, int M, int K, int N, const float* W, int k_per_split, int n_split,
                              float* part, cudaStream_t st);

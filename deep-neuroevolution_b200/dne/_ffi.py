@@ -35,6 +35,14 @@ class NetDesc(C.Structure):
                 ("layers", LayerDesc * DNE_MAX_LAYERS)]
 
 
+MAZE_MAX_WALLS = 64
+
+
+class MazeDesc(C.Structure):
+    _fields_ = [("n_walls", C.c_int32), ("collisions_stick", C.c_int32), ("goal", C.c_float * 2),
+                ("walls", (C.c_float * 4) * MAZE_MAX_WALLS)]
+
+
 class DneError(RuntimeError):
     pass
 
@@ -57,6 +65,10 @@ _SIGS = {
     "dne_pendulum_net_supported": [C.POINTER(NetDesc)],
     "dne_pendulum_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                               _P, _P, _P],
+    "dne_maze_net_supported": [C.POINTER(NetDesc)],
+    "dne_maze_episodes": [_P, C.POINTER(MazeDesc), C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P,
+                          _P, _P, _P, _P, _P, _P, _P],
+    "dne_abi_maze_size": [C.POINTER(C.c_int)],
     "dne_theta_prepare": [_P, C.POINTER(NetDesc), _P, C.c_int, _P, C.c_size_t, _P],
     "dne_theta_forget": [_P, _P],
     "dne_vbn_ws_bytes": [C.POINTER(NetDesc), C.c_int, C.c_int, C.POINTER(C.c_size_t)],
@@ -107,6 +119,9 @@ def lib():
         L.dne_abi_sizes(C.byref(a), C.byref(b))
         if (a.value, b.value) != (C.sizeof(LayerDesc), C.sizeof(NetDesc)):
             raise DneError(f"ABI mismatch: C structs {a.value}/{b.value} bytes, ctypes {C.sizeof(LayerDesc)}/{C.sizeof(NetDesc)}")
+        L.dne_abi_maze_size(C.byref(a))
+        if a.value != C.sizeof(MazeDesc):
+            raise DneError(f"ABI mismatch: C dne_maze_desc {a.value} bytes, ctypes {C.sizeof(MazeDesc)}")
         _lib = L
     return _lib
 

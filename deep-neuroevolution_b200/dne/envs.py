@@ -10,19 +10,21 @@ ALE / gym / MuJoCo are not vendored by the reference and are absent from this im
 here is the synthetic Frostbite-shaped stub the measurement plan names (SURVEY.md 8d): i.i.d. uint8 84x84x4
 observations from a fixed pool, rewards 10*Bernoulli(0.05), fixed or ragged episode lengths.  A real emulator
 plugs in by subclassing ``BatchEnv``.  Four real tasks need no emulator: CartPole-v1 (``CartPoleEnv``), Acrobot-v1
-(``AcrobotEnv``), MountainCar-v0 (``MountainCarEnv``) and Pendulum-v1 (``PendulumEnv``), whose episodes run whole on the
-device (``dne.rollout.EpisodeKernelRunner``).
+(``AcrobotEnv``), MountainCar-v0 (``MountainCarEnv``), Pendulum-v1 (``PendulumEnv``) and the reference's hard maze
+(``MazeEnv``), whose episodes run whole on the device (``dne.rollout.EpisodeKernelRunner``).
 
 An environment with device episodes (``device_episodes = True``) supplies ``state_dim``, ``initial_states(k)``,
 ``episode_net_supported(net)`` and ``launch_episodes(...)``; ``kernel_policy_io`` says whether its kernel also takes
 observation statistics, action noise and observation sums (MujocoPolicy), and ``host_step`` whether the per-tick
-``RolloutRunner`` can step it on the host instead.
+``RolloutRunner`` can step it on the host instead.  ``bc_dim`` (default ``state_dim``) is how many leading components of
+the final state form the 'final' behaviour characterisation.
 """
 from __future__ import annotations
 
 from typing import Optional, Sequence
 
 import ctypes as C
+import os
 
 import numpy as np
 import torch
@@ -431,6 +433,89 @@ def _make_pendulum(env_id, n_slots, seed=0, episode_len=None, **kw):
     return PendulumEnv(n_slots, seed=seed, **kw)
 
 
+class MazeEnv(BatchEnv):
+    """The hard maze of the reference's GPU path (``gym_tensorflow.make('maze', batch_size)``: gym_tensorflow/maze/maze.h
+    stepped as tf_maze.cpp does; DESIGN.md 3.7) for a whole population, stepped on the device in one launch of
+    ``dne_maze_episodes`` (``dne.rollout.EpisodeKernelRunner``).  A navigator with 6 rangefinders and a 4-sector goal
+    radar (11 float32 observations, the first a constant 1) and two continuous outputs (turn, speed), played for a fixed
+    400 steps; the only reward is -distance to the goal on the 400th step, so a truncated episode pays 0.  Every episode
+    starts from the maze file's start.  The state is (x, y, heading, speed, ang_vel, t, collided); the 'final' behaviour
+    characterisation is its first ``bc_dim`` = 2 components, the final (x, y) of the reference's ``MazeFinalState``.
+    ``maze_file``: a maze in the reference's text format (default: the reference's hard maze, tests/golden/hard_maze.txt).
+    There is no host step."""
+    device_episodes = True
+    host_step = False
+    kernel_policy_io = True
+    state_dim = 7
+    bc_dim = 2
+    MAX_STEPS = 400
+
+    def __init__(self, n_slots: int, maze_file: Optional[str] = None, seed: int = 0):
+        self.n_slots = int(n_slots)
+        self.maze_file = maze_file or DEFAULT_MAZE_FILE
+        self.walls, self.start, self.goal, self.collisions_stick = parse_maze(self.maze_file)
+        self.observation_space = Box(-np.inf, np.inf, (11,))
+        self.action_space = Box(-0.5, 0.5, (2,))
+        self.max_episode_steps = self.MAX_STEPS
+        self.desc = F.MazeDesc(n_walls=len(self.walls), collisions_stick=int(self.collisions_stick))
+        self.desc.goal[0], self.desc.goal[1] = self.goal
+        for j, w in enumerate(self.walls):
+            for k in range(4):
+                self.desc.walls[j][k] = float(w[k])
+
+    def initial_states(self, k: int) -> np.ndarray:
+        """float64 [k, 7]: the start, heading, speed and angular velocity 0, no steps taken, no collision."""
+        s = np.zeros((int(k), self.state_dim))
+        s[:, 0], s[:, 1] = self.start
+        return s
+
+    def episode_net_supported(self, net) -> bool:
+        return True                # the only path: the kernel itself rejects a net it cannot run
+
+    def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
+                        d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None):
+        F.check(F.lib().dne_maze_episodes(
+            ctx.handle, C.byref(self.desc), C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale),
+            F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise), F.ptr(d_ret),
+            F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq), F.stream_ptr()))
+
+    def _host_stepping(self, *a, **kw):
+        raise NotImplementedError("MazeEnv runs whole episodes on the device: use dne.rollout.make_runner "
+                                  "(EpisodeKernelRunner), not the per-tick host reset / step")
+    reset = step = obs_block = get_ram = _host_stepping
+
+
+DEFAULT_MAZE_FILE = os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "tests",
+                                 "golden", "hard_maze.txt")
+
+
+def parse_maze(path: str):
+    """A maze in the reference's text format (maze.h ``load_from``): the collision flag, the step count (unused: episodes
+    are 400 steps, as tf_maze.cpp fixes them), the wall count, the start (x, y), the start heading (unused: ``reset``
+    sets 0), the goal (x, y), a point of interest (unused), then one wall (ax, ay, bx, by) per line.  Returns (float32
+    walls [n, 4], start, goal, collision flag)."""
+    with open(path) as f:
+        tok = f.read().split()
+    try:
+        flag, n = int(tok[0]), int(tok[2])
+        v = [float(t) for t in tok[3:10 + 4 * n]]
+    except (IndexError, ValueError) as e:
+        raise ValueError(f"{path}: not a maze file ({e})") from None
+    if len(v) != 7 + 4 * n or n < 0:
+        raise ValueError(f"{path}: {n} walls announced, {max(len(v) - 7, 0) / 4:g} given")
+    if n > F.MAZE_MAX_WALLS:
+        raise ValueError(f"{path}: {n} walls, the device maze takes at most {F.MAZE_MAX_WALLS}")
+    f32 = np.float32
+    return (np.array(v[7:], dtype=np.float32).reshape(n, 4), (float(f32(v[0])), float(f32(v[1]))),
+            (float(f32(v[3])), float(f32(v[4]))), bool(flag))
+
+
+def _make_maze(env_id, n_slots, seed=0, episode_len=None, maze_file=None, **kw):
+    if episode_len is not None:
+        raise ValueError("the maze has a fixed 400-step episode; use the episode cutoff of the config instead")
+    return MazeEnv(n_slots, maze_file=maze_file, seed=seed)
+
+
 ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_len=, **kw) -> BatchEnv (real emulators plug in here)
     "CartPole-v1": _make_cartpole,
     "gym.CartPole-v1": _make_cartpole,   # the id of the reference GPU path's configurations/es_gym_config.json
@@ -439,4 +524,5 @@ ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_
     "gym.Acrobot-v1": _make_acrobot,
     "MountainCar-v0": _make_mountaincar,         # MountainCarContinuous-v0 does not match this prefix
     "gym.MountainCar-v0": _make_mountaincar,
+    "maze": _make_maze,                          # gym_tensorflow.make('maze', ...) of the reference GPU path
 }

@@ -253,7 +253,7 @@ class RolloutRunner:
 
 class EpisodeKernelRunner:
     """``RolloutRunner`` for environments whose episodes run entirely on the device (``env.device_episodes``:
-    ``dne.envs.CartPoleEnv``, ``AcrobotEnv``, ``MountainCarEnv``, ``PendulumEnv``): every member of every unit plays its whole episode inside ONE
+    ``dne.envs.CartPoleEnv``, ``AcrobotEnv``, ``MountainCarEnv``, ``PendulumEnv``, ``MazeEnv``): every member of every unit plays its whole episode inside ONE
     launch (``env.launch_episodes``), followed by one host sync for the results.  Same ``run`` signature and
     ``RolloutResult`` as ``RolloutRunner``.
 
@@ -277,7 +277,8 @@ class EpisodeKernelRunner:
     def run(self, theta: torch.Tensor, units: List[Unit], timestep_limit: Optional[int] = None, *, ob_mean=None,
             ob_std=None, collect_bc: Optional[str] = None, ac_noise_std: float = 0.0,
             random_stream: Optional[np.random.RandomState] = None, save_obs_prob: float = 0.0) -> RolloutResult:
-        """Evaluate every unit once.  ``collect_bc``: None | 'final' (float64 [env.state_dim] state after the last step)."""
+        """Evaluate every unit once.  ``collect_bc``: None | 'final' (float64 [env.bc_dim]: the leading components of the
+        state after the last step; ``bc_dim`` defaults to ``env.state_dim``)."""
         G, env = self.G, self.env
         if not env.kernel_policy_io:
             if ob_mean is not None or ob_std is not None:
@@ -351,7 +352,8 @@ class EpisodeKernelRunner:
         res.ticks = 1
         if d_fin is not None:
             fin = host["fin"].numpy().reshape(n_units, G, sd)
-            res.bcs = [[fin[u, g].copy() for g in range(G)] for u in range(n_units)]
+            bd = getattr(env, "bc_dim", sd)
+            res.bcs = [[fin[u, g, :bd].copy() for g in range(G)] for u in range(n_units)]
         if want_obstat:                       # the flagged members' sums, added in member order
             s_, q_ = host["ob_sum"].numpy(), host["ob_sumsq"].numpy()
             for m in np.nonzero(save)[0]:
@@ -366,8 +368,11 @@ def make_runner(ctx: F.Context, net: NetSpec, env: BatchEnv, action_fn=None, **k
     (``env.device_episodes``), the environment's kernel takes ``net`` (``env.episode_net_supported``) and no host
     ``action_fn`` maps the network's output to actions; otherwise the per-tick ``RolloutRunner`` when the environment
     has a host step.  ``action_fn``: the policy's map from output rows to actions (discretised MuJoCo heads), None for
-    the identity.  ``kw`` are ``RolloutRunner``'s arguments."""
+    the identity; an environment without a host step refuses one.  ``kw`` are ``RolloutRunner``'s arguments."""
     device = getattr(env, "device_episodes", False)
+    if device and action_fn is not None and not env.host_step:
+        raise NotImplementedError(f"{type(env).__name__} runs only on its episode kernel, whose head is the action: a "
+                                  "discretised ('uniform:' / 'custom:') head needs a host action map; use 'continuous:'")
     if device and ((action_fn is None and env.episode_net_supported(net)) or not env.host_step):
         r = EpisodeKernelRunner(ctx, net, env, **kw)
     else:

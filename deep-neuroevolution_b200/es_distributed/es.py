@@ -143,8 +143,10 @@ def setup(exp, single_threaded, n_slots=256, env=None, seed=None):
     from . import policies
     config = Config(**exp['config'])
     if env is None:
+        extra = {'maze_file': exp['maze_file']} if exp.get('maze_file') else {}
         env = make_env(exp['env_id'], n_slots, seed=0 if seed is None else seed,
-                       episode_len=exp.get('synthetic_episode_len'), allow_synthetic=bool(exp.get('allow_synthetic_env')))
+                       episode_len=exp.get('synthetic_episode_len'), allow_synthetic=bool(exp.get('allow_synthetic_env')),
+                       **extra)
     policy = getattr(policies, exp['policy']['type'])(env.observation_space, env.action_space, **exp['policy']['args'],
                                                      seed=seed)
     return config, env, None, policy

@@ -88,6 +88,8 @@ const char* dne_last_error(void);
 int         dne_version(void);
 /* ABI self-check for FFI bindings: sizeof(dne_layer_desc), sizeof(dne_net_desc). */
 int         dne_abi_sizes(int* layer_desc_bytes, int* net_desc_bytes);
+/* The same for sizeof(dne_maze_desc). */
+int         dne_abi_maze_size(int* maze_desc_bytes);
 
 /* ---- measurement hooks (bench.py) -------------------------------------------------------------------
  * dne_launch_count: kernels launched by this library in this process so far (reset != 0 zeroes it).
@@ -221,6 +223,34 @@ int dne_pendulum_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_
                           const double* d_init_state, int max_steps, const float* d_ob_mean, const float* d_ob_std,
                           const float* d_ac_noise, float* d_returns, float* d_signreturns, int32_t* d_lengths,
                           double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, void* stream);
+
+/* The hard maze of the reference's GPU path (gym_tensorflow/maze: maze.h stepped as tf_maze.cpp does; DESIGN.md 3.7):
+ * the walls as segments (ax, ay, bx, by), at most DNE_MAZE_MAX_WALLS; the goal; the maze file's collision flag (nonzero:
+ * a collision freezes the navigator for the rest of the episode; 0 in the hard maze). */
+#define DNE_MAZE_MAX_WALLS 64
+typedef struct {
+    int32_t n_walls;
+    int32_t collisions_stick;
+    float goal[2];
+    float walls[DNE_MAZE_MAX_WALLS][4];
+} dne_maze_desc;
+
+/* Hard-maze episodes run entirely on the device, one per member, for MujocoPolicy 'continuous:' nets.  Arguments as
+ * dne_pendulum_episodes, with: d_init_state / d_final_state double[n][7] = (x, y, heading, speed, ang_vel, t, collided),
+ * float32 values and t the steps already taken (the reset state is (start, 0, 0, 0, 0, 0)); 1 <= max_steps <= 400;
+ * observation float32[11] = (1, the 6 rangefinders / 100, the 4 goal-radar sectors); action = head[2] +
+ * d_ac_noise[m][step][0..1] (nullable [n][max_steps][2]), stepped as interpret_outputs(a0 + 0.5, a1 + 0.5) and Update();
+ * the reward is 0, and -distance to the goal on the step on which t reaches 400 (a shorter episode pays 0);
+ * d_ob_sum / d_ob_sumsq double[n][11].  The final (x, y) is the reference's MazeFinalState behaviour characterisation.
+ * `maze` with n_walls outside 0..DNE_MAZE_MAX_WALLS returns DNE_ERR_ARG.  Supported nets: as dne_pendulum_episodes with
+ * ob_dim 11 and n_out 2; anything else returns DNE_ERR_UNSUP with the reason in dne_last_error(), and
+ * dne_maze_net_supported answers the same question without launching (0 or DNE_ERR_UNSUP). */
+int dne_maze_net_supported(const dne_net_desc* net);
+int dne_maze_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_desc* net, const float* d_theta,
+                      const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx, int n_members,
+                      const double* d_init_state, int max_steps, const float* d_ob_mean, const float* d_ob_std,
+                      const float* d_ac_noise, float* d_returns, float* d_signreturns, int32_t* d_lengths,
+                      double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, void* stream);
 
 /* Observation statistics of the running normaliser (es.py:356-363 rollout_and_update_ob_stat; RunningStat es.py:26-48):
  * adds the observations d_obs[slot, :] (float32 [*, ob_dim], the unnormalised vectors fed to this tick's forward) of the m

@@ -603,6 +603,120 @@ extern "C" int dne_maze_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const 
     return DNE_OK;
 }
 
+// ---- one member per thread-block cluster (nets too wide for one CTA) ----
+static bool cluster_size_ok(int cluster) { return cluster == 0 || cluster == 2 || cluster == 4 || cluster == 8; }
+
+// `rc` from a cluster launch or geometry query with its reason, prefixed with `fn`
+static int cluster_fail(const char* fn, int rc, const char* why) {
+    if (rc == DNE_ERR_UNSUP)
+        dne_set_error("%s: net not supported by the cluster episode kernel: %s", fn, why);
+    else
+        dne_set_error("%s: launch setup failed (%d): %s", fn, rc, why);
+    return rc;
+}
+
+static int pendulum_cluster_net_check(const dne_net_desc* net, const char* fn) {
+    const char* why = "";
+    if (!dne_pendulum_cluster_net_supported(net, &why)) return cluster_fail(fn, DNE_ERR_UNSUP, why);
+    return DNE_OK;
+}
+
+static int maze_cluster_net_check(const dne_net_desc* net, const char* fn) {
+    const char* why = "";
+    if (!dne_maze_cluster_net_supported(net, &why)) return cluster_fail(fn, DNE_ERR_UNSUP, why);
+    return DNE_OK;
+}
+
+extern "C" int dne_pendulum_cluster_net_supported(const dne_net_desc* net) {
+    DNE_CHECK_ARG(net, "null net");
+    return pendulum_cluster_net_check(net, "dne_pendulum_cluster_net_supported");
+}
+
+extern "C" int dne_maze_cluster_net_supported(const dne_net_desc* net) {
+    DNE_CHECK_ARG(net, "null net");
+    return maze_cluster_net_check(net, "dne_maze_cluster_net_supported");
+}
+
+extern "C" int dne_pendulum_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry) {
+    DNE_CHECK_ARG(net && geometry, "null pointer");
+    DNE_CHECK_ARG(cluster_size_ok(cluster), "cluster must be 0 (automatic), 2, 4 or 8");
+    int rc = pendulum_cluster_net_check(net, "dne_pendulum_cluster_geometry");
+    if (rc) return rc;
+    const char* why = "";
+    rc = dne_pendulum_cluster_geometry(net, cluster, geometry, &why);
+    return rc ? cluster_fail("dne_pendulum_cluster_geometry", rc, why) : DNE_OK;
+}
+
+extern "C" int dne_maze_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry) {
+    DNE_CHECK_ARG(net && geometry, "null pointer");
+    DNE_CHECK_ARG(cluster_size_ok(cluster), "cluster must be 0 (automatic), 2, 4 or 8");
+    int rc = maze_cluster_net_check(net, "dne_maze_cluster_geometry");
+    if (rc) return rc;
+    const char* why = "";
+    rc = dne_maze_cluster_geometry(net, cluster, geometry, &why);
+    return rc ? cluster_fail("dne_maze_cluster_geometry", rc, why) : DNE_OK;
+}
+
+extern "C" int dne_pendulum_cluster_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                                             const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                             int n_members, const double* d_init_state, int max_steps,
+                                             const float* d_ob_mean, const float* d_ob_std, const float* d_ac_noise,
+                                             float* d_returns, float* d_signreturns, int32_t* d_lengths,
+                                             double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, int cluster,
+                                             void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_signreturns && d_lengths,
+                  "null pointer");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1 && max_steps <= 200, "max_steps outside 1..200 (Pendulum-v1's TimeLimit)");
+    DNE_CHECK_ARG((d_ob_mean == nullptr) == (d_ob_std == nullptr), "pass both d_ob_mean and d_ob_std or neither");
+    DNE_CHECK_ARG((d_ob_sum == nullptr) == (d_ob_sumsq == nullptr), "pass both d_ob_sum and d_ob_sumsq or neither");
+    DNE_CHECK_ARG(cluster_size_ok(cluster), "cluster must be 0 (automatic), 2, 4 or 8");
+    const int rc0 = pendulum_cluster_net_check(net, "dne_pendulum_cluster_episodes");
+    if (rc0) return rc0;
+    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
+    if (n_members == 0) return DNE_OK;
+    const char* why = "";
+    const int rc = dne_launch_pendulum_cluster_episodes(net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx,
+                                                        n_members, d_init_state, max_steps, d_ob_mean, d_ob_std,
+                                                        d_ac_noise, d_returns, d_signreturns, d_lengths, d_final_state,
+                                                        d_ob_sum, d_ob_sumsq, cluster, &why, (cudaStream_t)stream);
+    if (rc) return cluster_fail("dne_pendulum_cluster_episodes", rc, why);
+    DNE_LAUNCH_CHECK();
+    return DNE_OK;
+}
+
+extern "C" int dne_maze_cluster_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_desc* net,
+                                         const float* d_theta, const int64_t* d_noise_idx, const float* d_scale,
+                                         const int32_t* d_theta_idx, int n_members, const double* d_init_state,
+                                         int max_steps, const float* d_ob_mean, const float* d_ob_std,
+                                         const float* d_ac_noise, float* d_returns, float* d_signreturns,
+                                         int32_t* d_lengths, double* d_final_state, double* d_ob_sum,
+                                         double* d_ob_sumsq, int cluster, void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    DNE_CHECK_ARG(maze, "null maze");
+    DNE_CHECK_ARG(maze->n_walls >= 0 && maze->n_walls <= DNE_MAZE_MAX_WALLS, "maze n_walls outside 0..64");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_signreturns && d_lengths,
+                  "null pointer");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1 && max_steps <= 400, "max_steps outside 1..400 (the maze's episode length)");
+    DNE_CHECK_ARG((d_ob_mean == nullptr) == (d_ob_std == nullptr), "pass both d_ob_mean and d_ob_std or neither");
+    DNE_CHECK_ARG((d_ob_sum == nullptr) == (d_ob_sumsq == nullptr), "pass both d_ob_sum and d_ob_sumsq or neither");
+    DNE_CHECK_ARG(cluster_size_ok(cluster), "cluster must be 0 (automatic), 2, 4 or 8");
+    const int rc0 = maze_cluster_net_check(net, "dne_maze_cluster_episodes");
+    if (rc0) return rc0;
+    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
+    if (n_members == 0) return DNE_OK;
+    const char* why = "";
+    const int rc = dne_launch_maze_cluster_episodes(maze, net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx,
+                                                    n_members, d_init_state, max_steps, d_ob_mean, d_ob_std, d_ac_noise,
+                                                    d_returns, d_signreturns, d_lengths, d_final_state, d_ob_sum,
+                                                    d_ob_sumsq, cluster, &why, (cudaStream_t)stream);
+    if (rc) return cluster_fail("dne_maze_cluster_episodes", rc, why);
+    DNE_LAUNCH_CHECK();
+    return DNE_OK;
+}
+
 extern "C" int dne_perturb_forward_mlp(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
                                        const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
                                        const uint8_t* d_active, int n_slots, int paired, const float* d_obs,

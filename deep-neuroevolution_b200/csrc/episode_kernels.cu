@@ -48,6 +48,11 @@ static EpisodeNet make_episode_net(const dne_net_desc* net) {
     return en;
 }
 
+// Parameter j of a member: fl(theta[row][j] + fl(scale * noise[idx + j])), the rounding of every forward of the engine.
+__device__ __forceinline__ float member_weight(const float* th, const float* nz, float s, int j) {
+    return __fadd_rn(th[j], __fmul_rn(s, nz[j]));
+}
+
 // The member's weights, once per episode, by `nthr` threads starting at thread `t`.
 __device__ __forceinline__ void build_member_weights(float* w, const EpisodeNet& net, const float* __restrict__ theta,
                                                      const float* __restrict__ noise, const int64_t* __restrict__ noise_idx,
@@ -56,7 +61,7 @@ __device__ __forceinline__ void build_member_weights(float* w, const EpisodeNet&
     const float* th = theta + (theta_idx ? (int64_t)theta_idx[m] * net.P : 0);
     const float* nz = noise + noise_idx[m];
     const float s = scale[m];
-    for (int j = t; j < net.P; j += nthr) w[j] = __fadd_rn(th[j], __fmul_rn(s, nz[j]));
+    for (int j = t; j < net.P; j += nthr) w[j] = member_weight(th, nz, s, j);
 }
 
 // The checks both episode kernels share: dense layers only, chained widths, no batch norm, vector observations of
@@ -693,7 +698,7 @@ static ContinuousGeom continuous_geom(const dne_net_desc* net) {
 // weights plus its two activation buffers within one CTA's shared memory (for Pendulum hidden [200, 200] fits,
 // [256, 256] does not).  Any layer width runs: a group has at most 256 threads, each looping over its outputs.
 template <class Task>
-static bool continuous_net_supported(const dne_net_desc* net, const char** why) {
+static bool continuous_net_layers(const dne_net_desc* net, const char** why) {     // every check but the size
     if (!episode_net_common(net, DNE_MAX_LAYERS, Task::OB_DIM, Task::N_OUT, Task::OB_WHY, Task::OUT_WHY, why))
         return false;
     for (int l = 0; l < net->n_layers; ++l) {
@@ -703,6 +708,12 @@ static bool continuous_net_supported(const dne_net_desc* net, const char** why) 
             return false;
         }
     }
+    return true;
+}
+
+template <class Task>
+static bool continuous_net_supported(const dne_net_desc* net, const char** why) {
+    if (!continuous_net_layers<Task>(net, why)) return false;
     if (net->num_params > (1 << 24) || continuous_geom<Task>(net).member_bytes > CONT_SMEM_LIMIT) {
         *why = "one member's weights and activations exceed a CTA's shared memory (227 KB)";
         return false;
@@ -720,6 +731,62 @@ bool dne_maze_net_supported(const dne_net_desc* net, const char** why) {
 
 __device__ __forceinline__ void group_sync(int id, int nthr) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthr) : "memory");
+}
+
+// ---- the cluster kernel's per-step pieces (thread 0 of the member runs them): continuous_episode_kernel's code, which
+// keeps its own inline copy (routed through these helpers its maze instantiation compiles to other SASS, 0.3 % slower) ----
+// Observation component k as the first layer takes it, normalised as ob_norm_kernel; with `sums`, the unnormalised value
+// first goes into the member's float64 sums (ob_stat_accum_kernel's formula).
+__device__ __forceinline__ float ob_input(const float* o, int k, bool sums, double* os, double* oq,
+                                          const float* __restrict__ ob_mean, const float* __restrict__ ob_std) {
+    if (sums) {
+        os[k] = __dadd_rn(os[k], (double)o[k]);
+        oq[k] = __dadd_rn(oq[k], __dmul_rn((double)o[k], (double)o[k]));
+    }
+    return ob_mean ? fminf(fmaxf(__fdiv_rn(__fsub_rn(o[k], ob_mean[k]), ob_std[k]), -5.0f), 5.0f) : o[k];
+}
+
+// The linear head over the K inputs x (weights w[off_w + k * NO + j], bias w[off_b + j] unless off_b < 0), plus member
+// m's action noise of this step (ac_noise nullable, [n][max_steps][NO])
+template <int NO>
+__device__ __forceinline__ void linear_head(const float* x, const float* w, int off_w, int off_b, int K,
+                                            const float* __restrict__ ac_noise, int m, int max_steps, int step, float* a) {
+    const float* wl = w + off_w;
+#pragma unroll
+    for (int j = 0; j < NO; ++j) {
+        float acc = 0.0f;
+#pragma unroll 4
+        for (int k = 0; k < K; ++k) acc = fmaf(x[k], wl[k * NO + j], acc);
+        if (off_b >= 0) acc = __fadd_rn(acc, w[off_b + j]);
+        a[j] = ac_noise ? __fadd_rn(acc, ac_noise[((int64_t)m * max_steps + step) * NO + j]) : acc;
+    }
+}
+
+// The float32 reward into the float64 return and sign-return
+__device__ __forceinline__ void add_reward(float r, double& ret, double& sret) {
+    ret = __dadd_rn(ret, (double)r);
+    sret = __dadd_rn(sret, r > 0.0f ? 1.0 : r < 0.0f ? -1.0 : (double)r);    // np.sign (0 -> 0, NaN -> NaN)
+}
+
+// Member m's outputs
+template <class Task>
+__device__ __forceinline__ void store_member(const Task& env, int m, int max_steps, double ret, double sret,
+                                             const double* os, const double* oq, float* __restrict__ returns,
+                                             float* __restrict__ signreturns, int32_t* __restrict__ lengths,
+                                             double* __restrict__ final_state, double* __restrict__ ob_sum,
+                                             double* __restrict__ ob_sumsq) {
+    constexpr int OB = Task::OB_DIM;
+    returns[m] = __double2float_rn(ret);
+    signreturns[m] = __double2float_rn(sret);
+    lengths[m] = max_steps;
+    if (final_state) env.store(final_state + (int64_t)Task::STATE_DIM * m);
+    if (ob_sum) {
+#pragma unroll
+        for (int k = 0; k < OB; ++k) {
+            ob_sum[(int64_t)OB * m + k] = os[k];
+            ob_sumsq[(int64_t)OB * m + k] = oq[k];
+        }
+    }
 }
 
 // No spills (registers in DESIGN.md 3.6, 3.7).  Shared memory bounds the residency: for Pendulum hidden [64, 64] keeps
@@ -875,11 +942,7 @@ int dne_launch_pendulum_episodes(const dne_net_desc* net, const float* theta, co
                                            final_state, ob_sum, ob_sumsq, st);
 }
 
-int dne_launch_maze_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta, const float* noise,
-                             const int64_t* noise_idx, const float* scale, const int32_t* theta_idx, int n_members,
-                             const double* init_state, int max_steps, const float* ob_mean, const float* ob_std,
-                             const float* ac_noise, float* returns, float* signreturns, int32_t* lengths,
-                             double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st) {
+static MazeParams make_maze_params(const dne_maze_desc* maze) {
     MazeParams p = {};
     p.n_walls = maze->n_walls;
     p.sticky = maze->collisions_stick != 0;
@@ -895,7 +958,352 @@ int dne_launch_maze_episodes(const dne_maze_desc* maze, const dne_net_desc* net,
         p.ray_dx[i] = cosf(rad) * 100.0f;
         p.ray_dy[i] = sinf(rad) * 100.0f;
     }
-    return launch_continuous<MazeTask>(net, p, theta, noise, noise_idx, scale, theta_idx, n_members, init_state, max_steps,
-                                       ob_mean, ob_std, ac_noise, returns, signreturns, lengths, final_state, ob_sum,
-                                       ob_sumsq, st);
+    return p;
+}
+
+int dne_launch_maze_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta, const float* noise,
+                             const int64_t* noise_idx, const float* scale, const int32_t* theta_idx, int n_members,
+                             const double* init_state, int max_steps, const float* ob_mean, const float* ob_std,
+                             const float* ac_noise, float* returns, float* signreturns, int32_t* lengths,
+                             double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st) {
+    return launch_continuous<MazeTask>(net, make_maze_params(maze), theta, noise, noise_idx, scale, theta_idx, n_members,
+                                       init_state, max_steps, ob_mean, ob_std, ac_noise, returns, signreturns, lengths,
+                                       final_state, ob_sum, ob_sumsq, st);
+}
+
+// ---- continuous-action members too wide for one CTA: one member per thread-block cluster --------------------------------
+// MujocoPolicy's [256, 256] net (humanoid*.json) is 264-273 KiB of weights and activations, above a CTA's 227 KB.  Here
+// one member runs on a cluster of c in {2, 4, 8} CTAs (portable sizes), one group per CTA, and its weights are spread over
+// the cluster's shared memory (DSMEM, Hopper's distributed shared memory).  Layer l's N outputs are dealt to the ranks in
+// contiguous slices of S = ceil(N / c) (the last slices shorter or empty): rank r keeps its columns of W_l compacted to
+// [K][S] (columns past its slice unused) and its slice of the bias; the linear head lives on rank 0.  Every output is
+// still one thread's sequential fmaf over all K inputs in index order, then + bias, then apply_act, from weights built
+// with the same fl(theta + fl(scale * noise)), so every operation, and every result, equals continuous_episode_kernel's.
+// The K reduction is never split: that would change the fmaf order.
+// Per step: rank 0's stepping threads form the observation and thread 0 pushes it, normalised, into every rank's input
+// buffer; each hidden layer's slice is pushed into every rank's output buffer (ping-pong); rank 0 runs the head, adds the
+// action noise and steps the task.  Remote stores are st.shared::cluster to mapa-translated addresses; the cluster
+// barrier is barrier.cluster.arrive.release / wait.acquire, so the stores before it are visible to every rank after it.
+constexpr int CLUSTER_MAX = 8;                        // the largest portable cluster size
+constexpr int CLUSTER_SIZES[3] = {2, 4, 8};
+
+struct ClusterNet {
+    EpisodeNet net;                                   // the layers as theta lays them out
+    int slice[DNE_MAX_LAYERS];                        // hidden layer l: outputs per rank, ceil(cout / c)
+    int woff[DNE_MAX_LAYERS];                         // hidden layer l: this rank's weights [cin][slice], then bias [slice]
+    int head_off;                                     // rank 0: the head's weights [cin][n_out], then bias [n_out]
+    int buf_off;                                      // the two activation buffers, act_pad floats each
+    int act_pad;                                      // the widest layer (or observation) rounded up to 32 floats
+};
+
+struct ClusterGeom {
+    ClusterNet cn;
+    int c;                                            // CTAs per member
+    int threads;                                      // threads per CTA: the widest slice rounded up to 32, at most 256
+    size_t smem;                                      // dynamic shared memory per CTA (every rank gets rank 0's size)
+};
+
+// The split of a net that passed continuous_net_layers over c ranks
+template <class Task>
+static ClusterGeom cluster_geom(const dne_net_desc* net, int c) {
+    ClusterGeom g;
+    g.c = c;
+    g.cn.net = make_episode_net(net);
+    int width = Task::OB_DIM, max_slice = 0, off = 0;
+    const int L = net->n_layers;
+    for (int l = 0; l < DNE_MAX_LAYERS; ++l) g.cn.slice[l] = g.cn.woff[l] = 0;
+    for (int l = 0; l < L; ++l) {
+        const int K = net->layers[l].cin, N = net->layers[l].cout;
+        width = width > N ? width : N;
+        if (l + 1 < L) {
+            const int S = (N + c - 1) / c;
+            g.cn.slice[l] = S;
+            g.cn.woff[l] = off;
+            off += (K + 1) * S;
+            max_slice = max_slice > S ? max_slice : S;
+        } else {
+            g.cn.head_off = off;
+            off += (K + 1) * N;
+        }
+    }
+    g.cn.buf_off = (off + 31) / 32 * 32;
+    g.cn.act_pad = (width + 31) / 32 * 32;
+    const int thr = (max_slice + 31) / 32 * 32;
+    g.threads = thr < 32 ? 32 : (thr > CONT_CTA_THREADS ? CONT_CTA_THREADS : thr);
+    g.smem = ((size_t)g.cn.buf_off + 2 * (size_t)g.cn.act_pad) * sizeof(float);
+    return g;
+}
+
+// Which nets the cluster kernel runs for Task: continuous_net_supported's, except that the size limit is on one rank's
+// slices at c = 8 (the smallest) instead of on the whole member.  Hidden [256, 256] runs (maze: 142 KB per CTA at c = 2),
+// [2048, 2048] does not (2.1 MB per CTA even at c = 8).
+template <class Task>
+static bool continuous_cluster_net_supported(const dne_net_desc* net, const char** why) {
+    if (!continuous_net_layers<Task>(net, why)) return false;
+    if (net->num_params > (1 << 24) || cluster_geom<Task>(net, CLUSTER_MAX).smem > CONT_SMEM_LIMIT) {
+        *why = "one rank's slice of the weights and the activations exceed a CTA's shared memory (227 KB) even split "
+               "over a cluster of 8";
+        return false;
+    }
+    return true;
+}
+
+bool dne_pendulum_cluster_net_supported(const dne_net_desc* net, const char** why) {
+    return continuous_cluster_net_supported<PendulumTask>(net, why);
+}
+
+bool dne_maze_cluster_net_supported(const dne_net_desc* net, const char** why) {
+    return continuous_cluster_net_supported<MazeTask>(net, why);
+}
+
+__device__ __forceinline__ uint32_t cluster_addr(const float* p, int rank) {   // p in rank `rank`'s shared memory
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"((uint32_t)__cvta_generic_to_shared(p)), "r"(rank));
+    return r;
+}
+
+__device__ __forceinline__ void cluster_store(const float* p, int rank, float v) {
+    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr(p, rank)), "f"(v) : "memory");
+}
+
+// Every thread of every CTA of the cluster; the stores (local or remote) before it are visible to all of them after it
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+template <class Task>
+__global__ void __launch_bounds__(CONT_CTA_THREADS)
+continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ typename Task::Params prm,
+                                  const float* __restrict__ theta, const float* __restrict__ noise,
+                                  const int64_t* __restrict__ noise_idx, const float* __restrict__ scale,
+                                  const int32_t* __restrict__ theta_idx, int n_members,
+                                  const double* __restrict__ init_state, int max_steps, const float* __restrict__ ob_mean,
+                                  const float* __restrict__ ob_std, const float* __restrict__ ac_noise,
+                                  float* __restrict__ returns, float* __restrict__ signreturns,
+                                  int32_t* __restrict__ lengths, double* __restrict__ final_state,
+                                  double* __restrict__ ob_sum, double* __restrict__ ob_sumsq) {
+    constexpr int OB = Task::OB_DIM, NO = Task::N_OUT;
+    extern __shared__ float ep_smem[];
+    uint32_t c, rank;
+    asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(c));
+    asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+    const int m = blockIdx.x / c;                     // cluster index = member: the exit below is uniform over the cluster
+    if (m >= n_members) return;                       // (before any access to a peer's shared memory)
+    const int t = threadIdx.x, threads = blockDim.x;
+    const EpisodeNet& net = cn.net;
+    const int L = net.n_layers;
+    float* w = ep_smem;
+    float* buf0 = ep_smem + cn.buf_off;
+    float* buf1 = buf0 + cn.act_pad;
+
+    {   // this rank's slices of the member's weights (rank 0: and the head), element for element build_member_weights'
+        const float* th = theta + (theta_idx ? (int64_t)theta_idx[m] * net.P : 0);
+        const float* nz = noise + noise_idx[m];
+        const float s = scale[m];
+        for (int l = 0; l + 1 < L; ++l) {
+            const int K = net.cin[l], N = net.cout[l], S = cn.slice[l], n0 = (int)rank * S;
+            const int ns = N - n0 < S ? N - n0 : S;   // <= 0: an empty slice
+            float* wl = w + cn.woff[l];
+            for (int i = t; i < K * ns; i += threads) {
+                const int k = i / ns, j = i - k * ns;
+                wl[k * S + j] = member_weight(th, nz, s, net.off_w[l] + k * N + n0 + j);
+            }
+            if (net.off_b[l] >= 0)
+                for (int j = t; j < ns; j += threads) wl[K * S + j] = member_weight(th, nz, s, net.off_b[l] + n0 + j);
+        }
+        if (rank == 0) {
+            const int K = net.cin[L - 1];
+            float* wh = w + cn.head_off;
+            for (int i = t; i < K * NO; i += threads) wh[i] = member_weight(th, nz, s, net.off_w[L - 1] + i);
+            if (net.off_b[L - 1] >= 0)
+                for (int j = t; j < NO; j += threads) wh[K * NO + j] = member_weight(th, nz, s, net.off_b[L - 1] + j);
+        }
+    }
+
+    const bool stepper = rank == 0 && t < Task::STEP_THREADS;
+    Task env;
+    double ret = 0.0, sret = 0.0;
+    double os[OB], oq[OB];
+#pragma unroll
+    for (int k = 0; k < OB; ++k) os[k] = oq[k] = 0.0;
+    if (stepper) env.load(init_state + (int64_t)Task::STATE_DIM * m);
+    // Every rank has started (its shared memory exists) and built its weights before the first remote store.
+    cluster_sync();
+    // Races: buffer b is read by the layer that takes it as input (every rank) and, when the last hidden layer wrote it,
+    // by rank 0's head.  Every write into b, local or remote, comes after a cluster barrier that follows every read of b:
+    // layer l writes the buffer layer l - 1 read, after layer l - 1's barrier; layer 0 writes buf1, which the previous
+    // step's last hidden layer or head read, before the observation barrier; the observation goes into buf0, whose last
+    // readers (a layer of the previous step, before that layer's barrier, or the head, by the thread that writes the
+    // observation) are done.
+    for (int step = 0; step < max_steps; ++step) {
+        if (stepper) {                                // the observation, normalised as ob_norm_kernel, to every rank
+            float o[OB];
+            env.ob(o, prm, t);
+            if (t == 0) {
+#pragma unroll
+                for (int k = 0; k < OB; ++k) {
+                    const float v = ob_input(o, k, ob_sum != nullptr, os, oq, ob_mean, ob_std);
+                    for (int q = 0; q < (int)c; ++q) cluster_store(buf0 + k, q, v);
+                }
+            }
+        }
+        cluster_sync();
+        const float* x = buf0;
+        float* y = buf1;
+        for (int l = 0; l + 1 < L; ++l) {             // hidden layers: this rank's slice, pushed to every rank
+            const int K = net.cin[l], S = cn.slice[l], n0 = (int)rank * S;
+            const int ns = net.cout[l] - n0 < S ? net.cout[l] - n0 : S;
+            const float* wl = w + cn.woff[l];
+            for (int j = t; j < ns; j += threads) {
+                float acc = 0.0f;
+#pragma unroll 4
+                for (int k = 0; k < K; ++k) acc = fmaf(x[k], wl[k * S + j], acc);
+                if (net.off_b[l] >= 0) acc = __fadd_rn(acc, wl[K * S + j]);
+                const float v = apply_act(acc, net.act[l]);
+                for (int q = 0; q < (int)c; ++q) cluster_store(y + n0 + j, q, v);
+            }
+            cluster_sync();
+            const float* nx = y;
+            y = (float*)x;
+            x = nx;
+        }
+        if (stepper) {                                // rank 0: the linear head, the action noise, the environment step
+            float a[NO];
+            if (t == 0)
+                linear_head<NO>(x, w, cn.head_off, net.off_b[L - 1] >= 0 ? cn.head_off + net.cin[L - 1] * NO : -1,
+                                net.cin[L - 1], ac_noise, m, max_steps, step, a);
+            if (Task::STEP_THREADS > 1) {
+#pragma unroll
+                for (int j = 0; j < NO; ++j) a[j] = __shfl_sync(0xffffffffu, a[j], 0);
+            }
+            const float r = env.step(a, prm, t);
+            if (t == 0) add_reward(r, ret, sret);
+        }
+    }
+    // No CTA leaves while a peer may still store into its shared memory.
+    cluster_sync();
+    if (rank == 0 && t == 0)
+        store_member(env, m, max_steps, ret, sret, os, oq, returns, signreturns, lengths, final_state, ob_sum, ob_sumsq);
+}
+
+// Clusters of g resident on the device at once (the members one launch keeps in flight)
+template <class Task>
+static cudaError_t cluster_residency(const ClusterGeom& g, int* clusters) {
+    auto kern = continuous_cluster_episode_kernel<Task>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CONT_SMEM_LIMIT);
+    if (e != cudaSuccess) return e;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)g.c;
+    attr[0].val.clusterDim.y = attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)g.c);
+    cfg.blockDim = dim3((unsigned)g.threads);
+    cfg.dynamicSmemBytes = g.smem;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaOccupancyMaxActiveClusters(clusters, (void*)kern, &cfg);
+}
+
+// The cluster size for `want` (0: automatic, else 2, 4 or 8; the caller checked the value and the net).  Automatic: among
+// the sizes whose slices fit a CTA, the one with the most members resident on the device; on a tie the smaller.
+template <class Task>
+static int choose_cluster(const dne_net_desc* net, int want, ClusterGeom* out, int* resident, const char** why) {
+    int best = 0;
+    for (int c : CLUSTER_SIZES) {
+        if (want && c != want) continue;
+        const ClusterGeom g = cluster_geom<Task>(net, c);
+        if (g.smem > CONT_SMEM_LIMIT) continue;
+        int k = 0;
+        if (cluster_residency<Task>(g, &k) != cudaSuccess) return DNE_ERR_CUDA;
+        if (k > best) {
+            best = k;
+            *out = g;
+        }
+    }
+    if (best == 0) {
+        *why = want ? "one rank's slice of the weights and the activations exceed a CTA's shared memory (227 KB) at this "
+                      "cluster size, or no such cluster fits the device"
+                    : "no cluster size fits the device";
+        return DNE_ERR_UNSUP;
+    }
+    *resident = best;
+    return DNE_OK;
+}
+
+template <class Task>
+static int cluster_geometry(const dne_net_desc* net, int cluster, int* out, const char** why) {
+    ClusterGeom g;
+    int resident = 0;
+    const int rc = choose_cluster<Task>(net, cluster, &g, &resident, why);
+    if (rc) return rc;
+    out[0] = g.c;
+    out[1] = g.threads;
+    out[2] = (int)g.smem;
+    out[3] = resident;
+    return DNE_OK;
+}
+
+int dne_pendulum_cluster_geometry(const dne_net_desc* net, int cluster, int* out, const char** why) {
+    return cluster_geometry<PendulumTask>(net, cluster, out, why);
+}
+
+int dne_maze_cluster_geometry(const dne_net_desc* net, int cluster, int* out, const char** why) {
+    return cluster_geometry<MazeTask>(net, cluster, out, why);
+}
+
+template <class Task>
+static int launch_continuous_cluster(const dne_net_desc* net, const typename Task::Params& prm, const float* theta,
+                                     const float* noise, const int64_t* noise_idx, const float* scale,
+                                     const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
+                                     const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
+                                     float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
+                                     double* ob_sumsq, int cluster, const char** why, cudaStream_t st) {
+    ClusterGeom g;
+    int resident = 0;
+    const int rc = choose_cluster<Task>(net, cluster, &g, &resident, why);
+    if (rc) return rc;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)g.c;
+    attr[0].val.clusterDim.y = attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)((int64_t)n_members * g.c));
+    cfg.blockDim = dim3((unsigned)g.threads);
+    cfg.dynamicSmemBytes = g.smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, continuous_cluster_episode_kernel<Task>, g.cn, prm, theta, noise,
+                                             noise_idx, scale, theta_idx, n_members, init_state, max_steps, ob_mean,
+                                             ob_std, ac_noise, returns, signreturns, lengths, final_state, ob_sum,
+                                             ob_sumsq);
+    DNE_LAUNCHED(1);
+    if (e != cudaSuccess) {
+        *why = cudaGetErrorString(e);
+        return DNE_ERR_CUDA;
+    }
+    return DNE_OK;
+}
+
+int dne_launch_pendulum_cluster_episodes(const dne_net_desc* net, const float* theta, const float* noise,
+                                         const int64_t* noise_idx, const float* scale, const int32_t* theta_idx,
+                                         int n_members, const double* init_state, int max_steps, const float* ob_mean,
+                                         const float* ob_std, const float* ac_noise, float* returns, float* signreturns,
+                                         int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq,
+                                         int cluster, const char** why, cudaStream_t st) {
+    return launch_continuous_cluster<PendulumTask>(net, NoParams{}, theta, noise, noise_idx, scale, theta_idx, n_members,
+                                                   init_state, max_steps, ob_mean, ob_std, ac_noise, returns, signreturns,
+                                                   lengths, final_state, ob_sum, ob_sumsq, cluster, why, st);
+}
+
+int dne_launch_maze_cluster_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta,
+                                     const float* noise, const int64_t* noise_idx, const float* scale,
+                                     const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
+                                     const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
+                                     float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
+                                     double* ob_sumsq, int cluster, const char** why, cudaStream_t st) {
+    return launch_continuous_cluster<MazeTask>(net, make_maze_params(maze), theta, noise, noise_idx, scale, theta_idx,
+                                               n_members, init_state, max_steps, ob_mean, ob_std, ac_noise, returns,
+                                               signreturns, lengths, final_state, ob_sum, ob_sumsq, cluster, why, st);
 }

@@ -116,6 +116,25 @@ int dne_launch_maze_episodes(const dne_maze_desc* maze, const dne_net_desc* net,
                              const double* init_state, int max_steps, const float* ob_mean, const float* ob_std,
                              const float* ac_noise, float* returns, float* signreturns, int32_t* lengths,
                              double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st);
+// episode_kernels.cu: the same episodes with one member per thread-block cluster (dne_*_cluster_episodes).  `cluster` is
+// 0 (automatic) or 2, 4, 8 (already checked); the geometry is int[4] = (cluster size, threads per CTA, shared bytes per
+// CTA, members resident on the device).  DNE_ERR_UNSUP sets `why`, as does a failed launch (DNE_ERR_CUDA).
+bool dne_pendulum_cluster_net_supported(const dne_net_desc* net, const char** why);
+bool dne_maze_cluster_net_supported(const dne_net_desc* net, const char** why);
+int dne_pendulum_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry, const char** why);
+int dne_maze_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry, const char** why);
+int dne_launch_pendulum_cluster_episodes(const dne_net_desc* net, const float* theta, const float* noise,
+                                         const int64_t* noise_idx, const float* scale, const int32_t* theta_idx,
+                                         int n_members, const double* init_state, int max_steps, const float* ob_mean,
+                                         const float* ob_std, const float* ac_noise, float* returns, float* signreturns,
+                                         int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq,
+                                         int cluster, const char** why, cudaStream_t st);
+int dne_launch_maze_cluster_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta,
+                                     const float* noise, const int64_t* noise_idx, const float* scale,
+                                     const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
+                                     const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
+                                     float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
+                                     double* ob_sumsq, int cluster, const char** why, cudaStream_t st);
 
 int dne_launch_theta_gemm_tc(const float* X, int M, int K, int N, const float* W, int k_per_split, int n_split,
                              float* part, cudaStream_t st);

@@ -69,6 +69,14 @@ _SIGS = {
     "dne_maze_episodes": [_P, C.POINTER(MazeDesc), C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P,
                           _P, _P, _P, _P, _P, _P, _P],
     "dne_abi_maze_size": [C.POINTER(C.c_int)],
+    "dne_pendulum_cluster_net_supported": [C.POINTER(NetDesc)],
+    "dne_maze_cluster_net_supported": [C.POINTER(NetDesc)],
+    "dne_pendulum_cluster_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P,
+                                      _P, _P, _P, _P, C.c_int, _P],
+    "dne_maze_cluster_episodes": [_P, C.POINTER(MazeDesc), C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P,
+                                  _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, _P],
+    "dne_pendulum_cluster_geometry": [C.POINTER(NetDesc), C.c_int, C.POINTER(C.c_int)],
+    "dne_maze_cluster_geometry": [C.POINTER(NetDesc), C.c_int, C.POINTER(C.c_int)],
     "dne_theta_prepare": [_P, C.POINTER(NetDesc), _P, C.c_int, _P, C.c_size_t, _P],
     "dne_theta_forget": [_P, _P],
     "dne_vbn_ws_bytes": [C.POINTER(NetDesc), C.c_int, C.c_int, C.POINTER(C.c_size_t)],
@@ -170,6 +178,14 @@ def ptr(t: Optional[torch.Tensor], dtype=None):
 
 def stream_ptr():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def cluster_geometry(task: str, net_desc, cluster: int = 0) -> dict:
+    """The launch geometry of ``dne_<task>_cluster_episodes`` (task 'pendulum' or 'maze') for a net on the current
+    device: cluster size, threads and dynamic shared memory bytes per CTA, members resident at once."""
+    g = (C.c_int * 4)()
+    check(getattr(lib(), f"dne_{task}_cluster_geometry")(C.byref(net_desc), int(cluster), g))
+    return {"cluster": g[0], "threads": g[1], "smem_bytes": g[2], "resident_members": g[3]}
 
 
 class Context:

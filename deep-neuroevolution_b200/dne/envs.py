@@ -392,10 +392,15 @@ class PendulumEnv(BatchEnv):
 
     def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
                         d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None):
-        F.check(F.lib().dne_pendulum_episodes(
-            ctx.handle, C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale), F.ptr(d_row), n,
-            F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise), F.ptr(d_ret), F.ptr(d_sret),
-            F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq), F.stream_ptr()))
+        """One member per CTA group (``dne_pendulum_episodes``) when the net fits a CTA, otherwise one member per
+        thread-block cluster (``dne_pendulum_cluster_episodes``, automatic size): the same numbers either way."""
+        args = (C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale), F.ptr(d_row), n,
+                F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise), F.ptr(d_ret),
+                F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq))
+        if self.episode_net_supported(net):
+            F.check(F.lib().dne_pendulum_episodes(ctx.handle, *args, F.stream_ptr()))
+        else:
+            F.check(F.lib().dne_pendulum_cluster_episodes(ctx.handle, *args, 0, F.stream_ptr()))
 
     def _write_obs(self, slots):
         th, thdot = self.state[slots, 0], self.state[slots, 1]
@@ -474,10 +479,17 @@ class MazeEnv(BatchEnv):
 
     def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
                         d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None):
-        F.check(F.lib().dne_maze_episodes(
-            ctx.handle, C.byref(self.desc), C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale),
-            F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise), F.ptr(d_ret),
-            F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq), F.stream_ptr()))
+        """One member per CTA group (``dne_maze_episodes``) when the net fits a CTA, otherwise one member per
+        thread-block cluster (``dne_maze_cluster_episodes``, automatic size; MujocoPolicy's hidden [256, 256]): the same
+        numbers either way.  A net neither kernel takes raises with the cluster entry's reason."""
+        L = F.lib()
+        args = (C.byref(self.desc), C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale),
+                F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise),
+                F.ptr(d_ret), F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq))
+        if L.dne_maze_net_supported(C.byref(net.desc)) == 0:
+            F.check(L.dne_maze_episodes(ctx.handle, *args, F.stream_ptr()))
+        else:
+            F.check(L.dne_maze_cluster_episodes(ctx.handle, *args, 0, F.stream_ptr()))
 
     def _host_stepping(self, *a, **kw):
         raise NotImplementedError("MazeEnv runs whole episodes on the device: use dne.rollout.make_runner "

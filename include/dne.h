@@ -215,7 +215,8 @@ int dne_discrete_episodes(dne_ctx* ctx, int env, const dne_net_desc* net, const 
  * the forward, dne_ob_stat_accumulate's formula, in step order).  Enqueued on `stream`, no host sync.
  * Supported nets: 1..DNE_MAX_LAYERS dense layers of any width, DNE_OB_VECTOR with ob_dim 3, n_out 1, tanh or ReLU hidden layers, a
  * linear head, no batch norm, and one member's weights plus two activation buffers in one CTA's shared memory (227 KB:
- * hidden [200, 200] runs, [256, 256] does not); anything else returns DNE_ERR_UNSUP with the reason in dne_last_error().
+ * hidden [200, 200] runs, [256, 256] does not: dne_pendulum_cluster_episodes runs it); anything else returns
+ * DNE_ERR_UNSUP with the reason in dne_last_error().
  * dne_pendulum_net_supported answers the same question without launching (0 or DNE_ERR_UNSUP). */
 int dne_pendulum_net_supported(const dne_net_desc* net);
 int dne_pendulum_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
@@ -251,6 +252,36 @@ int dne_maze_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_des
                       const double* d_init_state, int max_steps, const float* d_ob_mean, const float* d_ob_std,
                       const float* d_ac_noise, float* d_returns, float* d_signreturns, int32_t* d_lengths,
                       double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, void* stream);
+
+/* Pendulum-v1 and hard-maze episodes for nets too wide for one CTA (MujocoPolicy's hidden [256, 256]; DESIGN.md 3.8):
+ * one member per thread-block cluster of `cluster` CTAs, its hidden layers' outputs dealt to the CTAs in contiguous
+ * slices and the activations exchanged through distributed shared memory.  Arguments, outputs and numerics as
+ * dne_pendulum_episodes / dne_maze_episodes, plus `cluster`: 0 picks the size with the most members resident on the
+ * device (the smaller on a tie), 2, 4 or 8 forces it; anything else returns DNE_ERR_ARG, and a forced size whose slices
+ * do not fit a CTA returns DNE_ERR_UNSUP.  Every operation is the single-CTA kernel's, so for a net both run the
+ * outputs are bit-identical at every cluster size.  Supported nets: as dne_pendulum_episodes / dne_maze_episodes, with
+ * the size limit on one CTA's slice at cluster size 8 (hidden [256, 256] and [512, 512] run, [2048, 2048] does not);
+ * anything else returns DNE_ERR_UNSUP with the reason in dne_last_error().  dne_*_cluster_net_supported answers the same
+ * question without launching (0 or DNE_ERR_UNSUP).  The existing entry points above are unchanged: they still refuse a
+ * net that does not fit one CTA. */
+int dne_pendulum_cluster_net_supported(const dne_net_desc* net);
+int dne_maze_cluster_net_supported(const dne_net_desc* net);
+int dne_pendulum_cluster_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                                  const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                  int n_members, const double* d_init_state, int max_steps, const float* d_ob_mean,
+                                  const float* d_ob_std, const float* d_ac_noise, float* d_returns, float* d_signreturns,
+                                  int32_t* d_lengths, double* d_final_state, double* d_ob_sum, double* d_ob_sumsq,
+                                  int cluster, void* stream);
+int dne_maze_cluster_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_desc* net, const float* d_theta,
+                              const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx, int n_members,
+                              const double* d_init_state, int max_steps, const float* d_ob_mean, const float* d_ob_std,
+                              const float* d_ac_noise, float* d_returns, float* d_signreturns, int32_t* d_lengths,
+                              double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, int cluster, void* stream);
+/* The launch geometry those entries use for `net` and `cluster` on the current device: geometry[4] = (cluster size,
+ * threads per CTA, dynamic shared memory bytes per CTA, members resident on the device at once by
+ * cudaOccupancyMaxActiveClusters).  Errors as the episode entries. */
+int dne_pendulum_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry);
+int dne_maze_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry);
 
 /* Observation statistics of the running normaliser (es.py:356-363 rollout_and_update_ob_stat; RunningStat es.py:26-48):
  * adds the observations d_obs[slot, :] (float32 [*, ob_dim], the unnormalised vectors fed to this tick's forward) of the m

@@ -1,8 +1,10 @@
 """Pendulum-v1 throughput of the fused episode kernel (needs an H100).
 
-    python tools/pendulum_throughput.py [--launches 50] [--gens 10] [--per-tick-members 256] [--out FILE.json]
+    python tools/pendulum_throughput.py [--launches 50] [--gens 10] [--per-tick-members 256] [--hidden 256 256]
+                                        [--cluster {0,2,4,8}] [--out FILE.json]
 
-Reports, from one process, for configurations/pendulum_es.json (MujocoPolicy, 200-step episodes):
+Reports, from one process, for configurations/pendulum_es.json (MujocoPolicy, 200-step episodes; --hidden replaces its
+hidden_dims, e.g. the reference's humanoid [256, 256]):
   * the kernel time of dne_pendulum_episodes (CUDA events over --launches back-to-back launches after 3 warm-up launches,
     with observation statistics, action noise and per-member observation sums) and env-steps/s, at the config's
     population and at about 5000 members;
@@ -12,6 +14,10 @@ Reports, from one process, for configurations/pendulum_es.json (MujocoPolicy, 20
   * at the config's population, the wall-clock of one EpisodeKernelRunner.run() with statistics sampling and action
     noise, and of its host-side action-noise draw (randn + float32 scaling + copy to the device) alone (medians of 5);
   * the card's name and power limit, read in the same run.
+The kernel is dne_pendulum_episodes when the net fits one CTA, otherwise dne_pendulum_cluster_episodes at the automatic
+cluster size, as PendulumEnv launches it; --cluster forces the cluster entry at that size (0: automatic), and the kernel
+results then also report its geometry (cluster size, threads and shared bytes per CTA, resident members).  --gens 0
+skips the generation and the runner costs, --per-tick-members 0 the per-tick comparison.
 """
 import argparse
 import ctypes as C
@@ -42,7 +48,7 @@ def card():
     return {"name": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip() or q.stderr.strip()}
 
 
-def time_kernel(ctx, net, theta, n, launches, seed=0):
+def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
     dev = torch.device("cuda", 0)
     rs = np.random.RandomState(seed)
     P, T = net.num_params, 200
@@ -58,11 +64,16 @@ def time_kernel(ctx, net, theta, n, launches, seed=0):
     d_s, d_q = torch.empty(n, 3, dtype=torch.float64, device=dev), torch.empty(n, 3, dtype=torch.float64, device=dev)
     th = theta.contiguous()
 
+    args = (C.byref(net.desc), F.ptr(th), F.ptr(d_idx), F.ptr(d_sc), None, n, F.ptr(d_init), T, F.ptr(d_mean),
+            F.ptr(d_std), F.ptr(d_ac), F.ptr(d_ret), F.ptr(d_sret), F.ptr(d_len), None, F.ptr(d_s), F.ptr(d_q))
+    if cluster is None and F.lib().dne_pendulum_net_supported(C.byref(net.desc)) != 0:
+        cluster = 0                                   # PendulumEnv's choice for a net too wide for one CTA
+
     def launch():
-        F.check(F.lib().dne_pendulum_episodes(
-            ctx.handle, C.byref(net.desc), F.ptr(th), F.ptr(d_idx), F.ptr(d_sc), None, n, F.ptr(d_init), T, F.ptr(d_mean),
-            F.ptr(d_std), F.ptr(d_ac), F.ptr(d_ret), F.ptr(d_sret), F.ptr(d_len), None, F.ptr(d_s), F.ptr(d_q),
-            F.stream_ptr()))
+        if cluster is None:
+            F.check(F.lib().dne_pendulum_episodes(ctx.handle, *args, F.stream_ptr()))
+        else:
+            F.check(F.lib().dne_pendulum_cluster_episodes(ctx.handle, *args, cluster, F.stream_ptr()))
     for _ in range(3):
         launch()
     torch.cuda.synchronize()
@@ -73,7 +84,10 @@ def time_kernel(ctx, net, theta, n, launches, seed=0):
     b.record()
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / launches
-    return {"members": n, "launches": launches, "kernel_ms": ms, "env_steps_per_s": n * T / (ms * 1e-3)}
+    res = {"members": n, "launches": launches, "kernel_ms": ms, "env_steps_per_s": n * T / (ms * 1e-3)}
+    if cluster is not None:
+        res["cluster_geometry"] = F.cluster_geometry("pendulum", net.desc, cluster)
+    return res
 
 
 def per_tick_vs_kernel(ctx, net, theta, n, rounds=3):
@@ -125,6 +139,9 @@ def main():
     ap.add_argument("--launches", type=int, default=50)
     ap.add_argument("--gens", type=int, default=10)
     ap.add_argument("--per-tick-members", type=int, default=256)
+    ap.add_argument("--hidden", type=int, nargs="+", default=None, help="hidden_dims instead of the config's")
+    ap.add_argument("--cluster", type=int, choices=(0, 2, 4, 8), default=None,
+                    help="force dne_pendulum_cluster_episodes at this cluster size (0: automatic) in the kernel timings")
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
@@ -132,19 +149,25 @@ def main():
     with open(CONFIG) as f:
         exp = json.load(f)
     exp["config"]["snapshot_freq"] = 0
+    if args.hidden:
+        exp["policy"]["args"]["hidden_dims"] = args.hidden
+        out["hidden_dims"] = args.hidden
     cfg = exp["config"]
     ctx = ES.default_context()
     env = PendulumEnv(8, seed=0)
     pol = policies.MujocoPolicy(env.observation_space, env.action_space, seed=0, **exp["policy"]["args"])
     n_cfg = cfg["episodes_per_batch"] + 2 * -(-int(round(cfg["episodes_per_batch"] // 2 * cfg["eval_prob"])) // 2)
-    out["kernel_config_population"] = time_kernel(ctx, pol.net, pol.device_theta, n_cfg, args.launches)
-    out["kernel_5000"] = time_kernel(ctx, pol.net, pol.device_theta, 5000, args.launches)
-    gens = []
-    ES.run_master(None, None, exp, max_iterations=args.gens, env=env, seed=0,
-                  on_iteration=lambda it, st, ex: gens.append(st["TimeElapsedThisIter"]))
-    out["generation_wallclock_s_median"] = float(np.median(gens[1:])) if len(gens) > 1 else gens[0]
-    out["runner_costs"] = runner_costs(ctx, pol.net, pol.device_theta, cfg["episodes_per_batch"] // 2)
-    out["per_tick_vs_kernel"] = per_tick_vs_kernel(ctx, pol.net, pol.device_theta, args.per_tick_members)
+    out["kernel_config_population"] = time_kernel(ctx, pol.net, pol.device_theta, n_cfg, args.launches,
+                                                  cluster=args.cluster)
+    out["kernel_5000"] = time_kernel(ctx, pol.net, pol.device_theta, 5000, args.launches, cluster=args.cluster)
+    if args.gens > 0:
+        gens = []
+        ES.run_master(None, None, exp, max_iterations=args.gens, env=env, seed=0,
+                      on_iteration=lambda it, st, ex: gens.append(st["TimeElapsedThisIter"]))
+        out["generation_wallclock_s_median"] = float(np.median(gens[1:])) if len(gens) > 1 else gens[0]
+        out["runner_costs"] = runner_costs(ctx, pol.net, pol.device_theta, cfg["episodes_per_batch"] // 2)
+    if args.per_tick_members > 0:
+        out["per_tick_vs_kernel"] = per_tick_vs_kernel(ctx, pol.net, pol.device_theta, args.per_tick_members)
     out["card_after"] = card()
     print(json.dumps(out, indent=1))
     if args.out:

@@ -717,6 +717,99 @@ extern "C" int dne_maze_cluster_episodes(dne_ctx* ctx, const dne_maze_desc* maze
     return DNE_OK;
 }
 
+// ---- discretised heads ----
+static int pendulum_binned_net_check(const dne_net_desc* net, int n_bins, const char* fn) {
+    const char* why = "";
+    if (!dne_pendulum_binned_net_supported(net, n_bins, &why)) {
+        dne_set_error("%s: net not supported by the binned episode kernels: %s", fn, why);
+        return DNE_ERR_UNSUP;
+    }
+    return DNE_OK;
+}
+
+static int maze_binned_net_check(const dne_net_desc* net, int n_bins, const char* fn) {
+    const char* why = "";
+    if (!dne_maze_binned_net_supported(net, n_bins, &why)) {
+        dne_set_error("%s: net not supported by the binned episode kernels: %s", fn, why);
+        return DNE_ERR_UNSUP;
+    }
+    return DNE_OK;
+}
+
+extern "C" int dne_pendulum_binned_net_supported(const dne_net_desc* net, int n_bins) {
+    DNE_CHECK_ARG(net, "null net");
+    return pendulum_binned_net_check(net, n_bins, "dne_pendulum_binned_net_supported");
+}
+
+extern "C" int dne_maze_binned_net_supported(const dne_net_desc* net, int n_bins) {
+    DNE_CHECK_ARG(net, "null net");
+    return maze_binned_net_check(net, n_bins, "dne_maze_binned_net_supported");
+}
+
+extern "C" int dne_pendulum_binned_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                                            const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                            int n_members, const double* d_init_state, int max_steps,
+                                            const float* d_ob_mean, const float* d_ob_std, const float* d_ac_noise,
+                                            float* d_returns, float* d_signreturns, int32_t* d_lengths,
+                                            double* d_final_state, double* d_ob_sum, double* d_ob_sumsq,
+                                            const float* bin_values_host, int n_bins, int cluster, void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_signreturns && d_lengths,
+                  "null pointer");
+    DNE_CHECK_ARG(bin_values_host, "null bin_values_host (the [1][n_bins] table of bin values)");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1 && max_steps <= 200, "max_steps outside 1..200 (Pendulum-v1's TimeLimit)");
+    DNE_CHECK_ARG((d_ob_mean == nullptr) == (d_ob_std == nullptr), "pass both d_ob_mean and d_ob_std or neither");
+    DNE_CHECK_ARG((d_ob_sum == nullptr) == (d_ob_sumsq == nullptr), "pass both d_ob_sum and d_ob_sumsq or neither");
+    DNE_CHECK_ARG(cluster_size_ok(cluster), "cluster must be 0 (automatic), 2, 4 or 8");
+    const int rc0 = pendulum_binned_net_check(net, n_bins, "dne_pendulum_binned_episodes");
+    if (rc0) return rc0;
+    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
+    if (n_members == 0) return DNE_OK;
+    const char* why = "";
+    const int rc = dne_launch_pendulum_binned_episodes(net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx,
+                                                       n_members, d_init_state, max_steps, d_ob_mean, d_ob_std, d_ac_noise,
+                                                       d_returns, d_signreturns, d_lengths, d_final_state, d_ob_sum,
+                                                       d_ob_sumsq, bin_values_host, n_bins, cluster, &why,
+                                                       (cudaStream_t)stream);
+    if (rc) return cluster_fail("dne_pendulum_binned_episodes", rc, why);
+    DNE_LAUNCH_CHECK();
+    return DNE_OK;
+}
+
+extern "C" int dne_maze_binned_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_desc* net,
+                                        const float* d_theta, const int64_t* d_noise_idx, const float* d_scale,
+                                        const int32_t* d_theta_idx, int n_members, const double* d_init_state,
+                                        int max_steps, const float* d_ob_mean, const float* d_ob_std,
+                                        const float* d_ac_noise, float* d_returns, float* d_signreturns,
+                                        int32_t* d_lengths, double* d_final_state, double* d_ob_sum, double* d_ob_sumsq,
+                                        const float* bin_values_host, int n_bins, int cluster, void* stream) {
+    DNE_CHECK_ARG(ctx && ctx->noise, "noise table not bound (dne_noise_bind)");
+    DNE_CHECK_ARG(maze, "null maze");
+    DNE_CHECK_ARG(maze->n_walls >= 0 && maze->n_walls <= DNE_MAZE_MAX_WALLS, "maze n_walls outside 0..64");
+    DNE_CHECK_ARG(net && d_theta && d_noise_idx && d_scale && d_init_state && d_returns && d_signreturns && d_lengths,
+                  "null pointer");
+    DNE_CHECK_ARG(bin_values_host, "null bin_values_host (the [2][n_bins] table of bin values)");
+    DNE_CHECK_ARG(n_members >= 0, "n_members < 0");
+    DNE_CHECK_ARG(max_steps >= 1 && max_steps <= 400, "max_steps outside 1..400 (the maze's episode length)");
+    DNE_CHECK_ARG((d_ob_mean == nullptr) == (d_ob_std == nullptr), "pass both d_ob_mean and d_ob_std or neither");
+    DNE_CHECK_ARG((d_ob_sum == nullptr) == (d_ob_sumsq == nullptr), "pass both d_ob_sum and d_ob_sumsq or neither");
+    DNE_CHECK_ARG(cluster_size_ok(cluster), "cluster must be 0 (automatic), 2, 4 or 8");
+    const int rc0 = maze_binned_net_check(net, n_bins, "dne_maze_binned_episodes");
+    if (rc0) return rc0;
+    DNE_CHECK_ARG(net->num_params <= ctx->noise_count, "net larger than the noise table");
+    if (n_members == 0) return DNE_OK;
+    const char* why = "";
+    const int rc = dne_launch_maze_binned_episodes(maze, net, d_theta, ctx->noise, d_noise_idx, d_scale, d_theta_idx,
+                                                   n_members, d_init_state, max_steps, d_ob_mean, d_ob_std, d_ac_noise,
+                                                   d_returns, d_signreturns, d_lengths, d_final_state, d_ob_sum,
+                                                   d_ob_sumsq, bin_values_host, n_bins, cluster, &why,
+                                                   (cudaStream_t)stream);
+    if (rc) return cluster_fail("dne_maze_binned_episodes", rc, why);
+    DNE_LAUNCH_CHECK();
+    return DNE_OK;
+}
+
 extern "C" int dne_perturb_forward_mlp(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
                                        const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
                                        const uint8_t* d_active, int n_slots, int paired, const float* d_obs,

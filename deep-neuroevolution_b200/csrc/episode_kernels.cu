@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include "forward.cuh"
 #include <math_constants.h>
+#include <type_traits>
 
 constexpr int EP_WARPS = 8;                 // discrete tasks: members per CTA (one per warp)
 constexpr int EP_MAX_WIDTH = 32;            // discrete tasks: every layer width fits one warp: lane j owns output j
@@ -445,6 +446,7 @@ struct PendulumTask {
     static constexpr int OB_DIM = 3, N_OUT = 1, STATE_DIM = 2, TIME_LIMIT = 200, STEP_THREADS = 1;
     static constexpr const char* OB_WHY = "Pendulum observations have ob_dim 3";
     static constexpr const char* OUT_WHY = "Pendulum has one continuous action (n_out 1)";
+    static constexpr const char* BIN_OUT_WHY = "Pendulum's binned head scores n_bins bins of its one action (n_out n_bins)";
     using Params = NoParams;
     double th = 0.0, thdot = 0.0;
 
@@ -521,6 +523,8 @@ struct MazeTask {
     static constexpr int OB_DIM = 11, N_OUT = 2, STATE_DIM = 7, TIME_LIMIT = 400, STEP_THREADS = 32;
     static constexpr const char* OB_WHY = "maze observations have ob_dim 11";
     static constexpr const char* OUT_WHY = "the maze has two continuous actions (n_out 2)";
+    static constexpr const char* BIN_OUT_WHY = "the maze's binned head scores n_bins bins of each of its two actions "
+                                               "(n_out 2 * n_bins)";
     using Params = MazeParams;
     float x = 0.f, y = 0.f, heading = 0.f, speed = 0.f, ang_vel = 0.f;
     int t = 0;
@@ -676,6 +680,87 @@ struct MazeTask {
     }
 };
 
+// ---- discretised heads (MujocoPolicy 'uniform:N' / 'custom:v0,..,vk'; DESIGN.md 3.9) ----------------------------------
+// The net scores N_OUT * nb bins, score d * nb + b being bin b of action dimension d; per dimension the action is the
+// value of the bin with the highest score (the first NaN if any score is NaN, otherwise the first maximum: numpy's
+// argmax), then the action noise is added.  The kernels take the head mode at compile time: BINNED = false is the linear
+// head, whose parameters stay the task's own, so those instantiations are unchanged.
+constexpr int BIN_MAX = 32;                           // bins per action dimension: one dimension's bins fit one warp
+
+template <class Task>
+struct BinnedParams {
+    typename Task::Params task;
+    float values[Task::N_OUT][BIN_MAX];               // the policy's bin table: values[d][b], b < nb
+    int nb;
+};
+
+template <class Task, bool BINNED>
+using EpisodeParams = typename std::conditional<BINNED, BinnedParams<Task>, typename Task::Params>::type;
+
+template <class Task>
+__device__ __forceinline__ const typename Task::Params& task_params(const typename Task::Params& p) { return p; }
+template <class Task>
+__device__ __forceinline__ const typename Task::Params& task_params(const BinnedParams<Task>& p) { return p.task; }
+
+// The chosen bin of one action dimension, in every lane of the warp; lane b < nb holds bin b's score s.  "The first NaN,
+// otherwise the first maximum" is the maximum under a total order (NaN above every number, then the larger value, then
+// the smaller index), so a shuffle butterfly finds it in 5 rounds whatever the pairing.  Lanes past nb hold -inf with a
+// larger index: they never win.
+__device__ __forceinline__ int warp_bin_argmax(float s, int lane, int nb) {
+    float v = lane < nb ? s : -CUDART_INF_F;
+    int i = lane;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, v, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, i, off);
+        const bool vn = v != v, on = ov != ov;
+        if (vn != on ? on : (vn || ov == v ? oi < i : ov > v)) {
+            v = ov;
+            i = oi;
+        }
+    }
+    return i;
+}
+
+// The binned head's scores: score j = sequential fmaf over the K inputs x in index order, then + bias (the linear head's
+// operations), thread t of `threads` computing scores t, t + threads, ...; the weights are [K][NS] at wl, the bias at bl
+// (nullptr: none).
+__device__ __forceinline__ void bin_scores(const float* x, const float* wl, const float* bl, int K, int NS, float* y,
+                                           int t, int threads) {
+    for (int j = t; j < NS; j += threads) {
+        float acc = 0.0f;
+#pragma unroll 4
+        for (int k = 0; k < K; ++k) acc = fmaf(x[k], wl[k * NS + j], acc);
+        if (bl) acc = __fadd_rn(acc, bl[j]);
+        y[j] = acc;
+    }
+}
+
+// Warp 0 of the member, after the scores are in y: every lane takes each dimension's bin, its value and member m's action
+// noise of this step (ac_noise nullable, [n][max_steps][N_OUT]); the lanes below Task::STEP_THREADS then step the task.
+template <class Task>
+__device__ __forceinline__ void binned_act_and_step(Task& env, const BinnedParams<Task>& prm, const float* y, int t,
+                                                    const float* __restrict__ ac_noise, int m, int max_steps, int step,
+                                                    double& ret, double& sret) {
+    constexpr int NO = Task::N_OUT;
+    const int nb = prm.nb;
+    float a[NO];
+#pragma unroll
+    for (int d = 0; d < NO; ++d) {
+        const int b = warp_bin_argmax(t < nb ? y[d * nb + t] : 0.0f, t, nb);
+        a[d] = prm.values[d][b];
+        if (ac_noise) a[d] = __fadd_rn(a[d], ac_noise[((int64_t)m * max_steps + step) * NO + d]);
+    }
+    __syncwarp();                                     // every lane's reads of y before any later write into it
+    if (t < Task::STEP_THREADS) {
+        const float r = env.step(a, prm.task, t);
+        if (t == 0) {
+            ret = __dadd_rn(ret, (double)r);
+            sret = __dadd_rn(sret, r > 0.0f ? 1.0 : r < 0.0f ? -1.0 : (double)r);
+        }
+    }
+}
+
 struct ContinuousGeom {
     int threads;                                      // threads per member: min(max layer width, 256), a multiple of 32
     int act_pad;                                      // floats of one activation buffer: max layer width rounded up to 32
@@ -697,10 +782,11 @@ static ContinuousGeom continuous_geom(const dne_net_desc* net) {
 // dimension Task::OB_DIM, Task::N_OUT outputs, tanh or ReLU hidden layers, a linear head, no batch norm, and one member's
 // weights plus its two activation buffers within one CTA's shared memory (for Pendulum hidden [200, 200] fits,
 // [256, 256] does not).  Any layer width runs: a group has at most 256 threads, each looping over its outputs.
+// A binned head checks the same with n_out = Task::N_OUT * nb.
 template <class Task>
-static bool continuous_net_layers(const dne_net_desc* net, const char** why) {     // every check but the size
-    if (!episode_net_common(net, DNE_MAX_LAYERS, Task::OB_DIM, Task::N_OUT, Task::OB_WHY, Task::OUT_WHY, why))
-        return false;
+static bool continuous_net_layers(const dne_net_desc* net, const char** why, int n_out = Task::N_OUT,
+                                  const char* out_why = Task::OUT_WHY) {     // every check but the size
+    if (!episode_net_common(net, DNE_MAX_LAYERS, Task::OB_DIM, n_out, Task::OB_WHY, out_why, why)) return false;
     for (int l = 0; l < net->n_layers; ++l) {
         const int act = net->layers[l].act;
         if (l == net->n_layers - 1 ? act != DNE_ACT_NONE : (act != DNE_ACT_TANH && act != DNE_ACT_RELU)) {
@@ -791,9 +877,11 @@ __device__ __forceinline__ void store_member(const Task& env, int m, int max_ste
 
 // No spills (registers in DESIGN.md 3.6, 3.7).  Shared memory bounds the residency: for Pendulum hidden [64, 64] keeps
 // 12 members (24 warps) per SM, [128, 128] 3, [200, 200] 1.
-template <class Task>
+// BINNED: the head is discretised (BinnedParams): every thread of the group computes its scores into the free activation
+// buffer, one more group barrier, then warp 0 picks the bins (binned_act_and_step).
+template <class Task, bool BINNED>
 __global__ void __launch_bounds__(CONT_CTA_THREADS)
-continuous_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, const __grid_constant__ typename Task::Params prm,
+continuous_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, const __grid_constant__ EpisodeParams<Task, BINNED> prm,
                           const float* __restrict__ theta, const float* __restrict__ noise,
                           const int64_t* __restrict__ noise_idx, const float* __restrict__ scale,
                           const int32_t* __restrict__ theta_idx, int n_members, const double* __restrict__ init_state,
@@ -824,7 +912,7 @@ continuous_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, 
     for (int step = 0; step < max_steps; ++step) {
         if (t < Task::STEP_THREADS) {         // the observation, normalised as ob_norm_kernel
             float o[OB];
-            env.ob(o, prm, t);
+            env.ob(o, task_params<Task>(prm), t);
             if (t == 0) {
 #pragma unroll
                 for (int k = 0; k < OB; ++k) {
@@ -857,7 +945,13 @@ continuous_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, 
             y = (float*)x;
             x = nx;
         }
-        if (t < Task::STEP_THREADS) {         // the linear head, the action noise, the environment step
+        if constexpr (BINNED) {               // the scores into y, which no thread reads again this step
+            const int NS = net.cout[L - 1];
+            bin_scores(x, w + net.off_w[L - 1], net.off_b[L - 1] >= 0 ? w + net.off_b[L - 1] : nullptr,
+                       net.cin[L - 1], NS, y, t, threads);
+            group_sync(bar, threads);
+            if (t < 32) binned_act_and_step(env, prm, y, t, ac_noise, m, max_steps, step, ret, sret);
+        } else if (t < Task::STEP_THREADS) {  // the linear head, the action noise, the environment step
             float a[NO];
             if (t == 0) {
                 const int K = net.cin[L - 1];
@@ -897,15 +991,15 @@ continuous_episode_kernel(EpisodeNet net, int threads, int act_pad, int groups, 
     }
 }
 
-template <class Task>
-static int launch_continuous(const dne_net_desc* net, const typename Task::Params& prm, const float* theta,
+template <class Task, bool BINNED = false>
+static int launch_continuous(const dne_net_desc* net, const EpisodeParams<Task, BINNED>& prm, const float* theta,
                              const float* noise, const int64_t* noise_idx, const float* scale, const int32_t* theta_idx,
                              int n_members, const double* init_state, int max_steps, const float* ob_mean,
                              const float* ob_std, const float* ac_noise, float* returns, float* signreturns,
                              int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq, cudaStream_t st) {
     const EpisodeNet en = make_episode_net(net);
     const ContinuousGeom g = continuous_geom<Task>(net);
-    auto kern = continuous_episode_kernel<Task>;
+    auto kern = continuous_episode_kernel<Task, BINNED>;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CONT_SMEM_LIMIT) != cudaSuccess)
         return DNE_ERR_CUDA;
     // members per CTA: the count that keeps the most members resident per SM (registers, shared memory, threads, as the
@@ -1071,9 +1165,12 @@ __device__ __forceinline__ void cluster_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <class Task>
+// BINNED: rank 0 keeps the discretised head's [cin][n_out] weights; its threads compute the scores into its free buffer,
+// one CTA barrier, then its warp 0 picks the bins (binned_act_and_step).  The other ranks go on to the next observation's
+// cluster barrier, which rank 0 reaches after its step, so nothing is stored into rank 0's buffers meanwhile.
+template <class Task, bool BINNED>
 __global__ void __launch_bounds__(CONT_CTA_THREADS)
-continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ typename Task::Params prm,
+continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ EpisodeParams<Task, BINNED> prm,
                                   const float* __restrict__ theta, const float* __restrict__ noise,
                                   const int64_t* __restrict__ noise_idx, const float* __restrict__ scale,
                                   const int32_t* __restrict__ theta_idx, int n_members,
@@ -1112,11 +1209,11 @@ continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ typenam
                 for (int j = t; j < ns; j += threads) wl[K * S + j] = member_weight(th, nz, s, net.off_b[l] + n0 + j);
         }
         if (rank == 0) {
-            const int K = net.cin[L - 1];
+            const int K = net.cin[L - 1], NH = BINNED ? net.cout[L - 1] : NO;
             float* wh = w + cn.head_off;
-            for (int i = t; i < K * NO; i += threads) wh[i] = member_weight(th, nz, s, net.off_w[L - 1] + i);
+            for (int i = t; i < K * NH; i += threads) wh[i] = member_weight(th, nz, s, net.off_w[L - 1] + i);
             if (net.off_b[L - 1] >= 0)
-                for (int j = t; j < NO; j += threads) wh[K * NO + j] = member_weight(th, nz, s, net.off_b[L - 1] + j);
+                for (int j = t; j < NH; j += threads) wh[K * NH + j] = member_weight(th, nz, s, net.off_b[L - 1] + j);
         }
     }
 
@@ -1138,7 +1235,7 @@ continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ typenam
     for (int step = 0; step < max_steps; ++step) {
         if (stepper) {                                // the observation, normalised as ob_norm_kernel, to every rank
             float o[OB];
-            env.ob(o, prm, t);
+            env.ob(o, task_params<Task>(prm), t);
             if (t == 0) {
 #pragma unroll
                 for (int k = 0; k < OB; ++k) {
@@ -1167,7 +1264,15 @@ continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ typenam
             y = (float*)x;
             x = nx;
         }
-        if (stepper) {                                // rank 0: the linear head, the action noise, the environment step
+        if constexpr (BINNED) {
+            if (rank == 0) {
+                const int K = net.cin[L - 1], NS = net.cout[L - 1];
+                bin_scores(x, w + cn.head_off, net.off_b[L - 1] >= 0 ? w + cn.head_off + K * NS : nullptr, K, NS, y, t,
+                           threads);
+                __syncthreads();                      // rank 0's CTA only
+                if (t < 32) binned_act_and_step(env, prm, y, t, ac_noise, m, max_steps, step, ret, sret);
+            }
+        } else if (stepper) {                         // rank 0: the linear head, the action noise, the environment step
             float a[NO];
             if (t == 0)
                 linear_head<NO>(x, w, cn.head_off, net.off_b[L - 1] >= 0 ? cn.head_off + net.cin[L - 1] * NO : -1,
@@ -1187,9 +1292,9 @@ continuous_cluster_episode_kernel(ClusterNet cn, const __grid_constant__ typenam
 }
 
 // Clusters of g resident on the device at once (the members one launch keeps in flight)
-template <class Task>
+template <class Task, bool BINNED>
 static cudaError_t cluster_residency(const ClusterGeom& g, int* clusters) {
-    auto kern = continuous_cluster_episode_kernel<Task>;
+    auto kern = continuous_cluster_episode_kernel<Task, BINNED>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CONT_SMEM_LIMIT);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
@@ -1207,7 +1312,7 @@ static cudaError_t cluster_residency(const ClusterGeom& g, int* clusters) {
 
 // The cluster size for `want` (0: automatic, else 2, 4 or 8; the caller checked the value and the net).  Automatic: among
 // the sizes whose slices fit a CTA, the one with the most members resident on the device; on a tie the smaller.
-template <class Task>
+template <class Task, bool BINNED = false>
 static int choose_cluster(const dne_net_desc* net, int want, ClusterGeom* out, int* resident, const char** why) {
     int best = 0;
     for (int c : CLUSTER_SIZES) {
@@ -1215,7 +1320,7 @@ static int choose_cluster(const dne_net_desc* net, int want, ClusterGeom* out, i
         const ClusterGeom g = cluster_geom<Task>(net, c);
         if (g.smem > CONT_SMEM_LIMIT) continue;
         int k = 0;
-        if (cluster_residency<Task>(g, &k) != cudaSuccess) return DNE_ERR_CUDA;
+        if (cluster_residency<Task, BINNED>(g, &k) != cudaSuccess) return DNE_ERR_CUDA;
         if (k > best) {
             best = k;
             *out = g;
@@ -1252,8 +1357,8 @@ int dne_maze_cluster_geometry(const dne_net_desc* net, int cluster, int* out, co
     return cluster_geometry<MazeTask>(net, cluster, out, why);
 }
 
-template <class Task>
-static int launch_continuous_cluster(const dne_net_desc* net, const typename Task::Params& prm, const float* theta,
+template <class Task, bool BINNED = false>
+static int launch_continuous_cluster(const dne_net_desc* net, const EpisodeParams<Task, BINNED>& prm, const float* theta,
                                      const float* noise, const int64_t* noise_idx, const float* scale,
                                      const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
                                      const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
@@ -1261,7 +1366,7 @@ static int launch_continuous_cluster(const dne_net_desc* net, const typename Tas
                                      double* ob_sumsq, int cluster, const char** why, cudaStream_t st) {
     ClusterGeom g;
     int resident = 0;
-    const int rc = choose_cluster<Task>(net, cluster, &g, &resident, why);
+    const int rc = choose_cluster<Task, BINNED>(net, cluster, &g, &resident, why);
     if (rc) return rc;
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];
@@ -1274,9 +1379,9 @@ static int launch_continuous_cluster(const dne_net_desc* net, const typename Tas
     cfg.stream = st;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, continuous_cluster_episode_kernel<Task>, g.cn, prm, theta, noise,
-                                             noise_idx, scale, theta_idx, n_members, init_state, max_steps, ob_mean,
-                                             ob_std, ac_noise, returns, signreturns, lengths, final_state, ob_sum,
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, continuous_cluster_episode_kernel<Task, BINNED>, g.cn, prm, theta,
+                                             noise, noise_idx, scale, theta_idx, n_members, init_state, max_steps,
+                                             ob_mean, ob_std, ac_noise, returns, signreturns, lengths, final_state, ob_sum,
                                              ob_sumsq);
     DNE_LAUNCHED(1);
     if (e != cudaSuccess) {
@@ -1306,4 +1411,80 @@ int dne_launch_maze_cluster_episodes(const dne_maze_desc* maze, const dne_net_de
     return launch_continuous_cluster<MazeTask>(net, make_maze_params(maze), theta, noise, noise_idx, scale, theta_idx,
                                                n_members, init_state, max_steps, ob_mean, ob_std, ac_noise, returns,
                                                signreturns, lengths, final_state, ob_sum, ob_sumsq, cluster, why, st);
+}
+
+// ---- discretised heads: one entry per task, the single-CTA kernel or a cluster ------------------------------------------
+// Which nets the binned entry runs for Task with nb bins per action dimension: continuous_net_layers' checks with n_out =
+// Task::N_OUT * nb, and the member within one CTA or, split, within a cluster of 8.
+template <class Task>
+static bool binned_net_supported(const dne_net_desc* net, int nb, const char** why) {
+    if (nb < 2 || nb > BIN_MAX) {
+        *why = "a binned head needs 2..32 bins per action dimension";
+        return false;
+    }
+    if (!continuous_net_layers<Task>(net, why, Task::N_OUT * nb, Task::BIN_OUT_WHY)) return false;
+    if (net->num_params > (1 << 24) || (continuous_geom<Task>(net).member_bytes > CONT_SMEM_LIMIT &&
+                                        cluster_geom<Task>(net, CLUSTER_MAX).smem > CONT_SMEM_LIMIT)) {
+        *why = "one rank's slice of the weights and the activations exceed a CTA's shared memory (227 KB) even split "
+               "over a cluster of 8";
+        return false;
+    }
+    return true;
+}
+
+bool dne_pendulum_binned_net_supported(const dne_net_desc* net, int nb, const char** why) {
+    return binned_net_supported<PendulumTask>(net, nb, why);
+}
+
+bool dne_maze_binned_net_supported(const dne_net_desc* net, int nb, const char** why) {
+    return binned_net_supported<MazeTask>(net, nb, why);
+}
+
+// cluster 0 with a member that fits one CTA: the single-CTA kernel; otherwise the cluster kernel at `cluster` (0:
+// automatic).  `bins` is the host table [N_OUT][nb], copied into the kernel's parameters.
+template <class Task>
+static int launch_binned(const dne_net_desc* net, const typename Task::Params& tp, const float* bins, int nb,
+                         const float* theta, const float* noise, const int64_t* noise_idx, const float* scale,
+                         const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
+                         const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
+                         float* signreturns, int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq,
+                         int cluster, const char** why, cudaStream_t st) {
+    BinnedParams<Task> prm = {};
+    prm.task = tp;
+    prm.nb = nb;
+    for (int d = 0; d < Task::N_OUT; ++d)
+        for (int b = 0; b < nb; ++b) prm.values[d][b] = bins[d * nb + b];
+    if (cluster == 0 && continuous_geom<Task>(net).member_bytes <= CONT_SMEM_LIMIT) {
+        const int rc = launch_continuous<Task, true>(net, prm, theta, noise, noise_idx, scale, theta_idx, n_members,
+                                                     init_state, max_steps, ob_mean, ob_std, ac_noise, returns,
+                                                     signreturns, lengths, final_state, ob_sum, ob_sumsq, st);
+        if (rc) *why = "the single-CTA kernel's attributes or occupancy could not be set";
+        return rc;
+    }
+    return launch_continuous_cluster<Task, true>(net, prm, theta, noise, noise_idx, scale, theta_idx, n_members,
+                                                 init_state, max_steps, ob_mean, ob_std, ac_noise, returns, signreturns,
+                                                 lengths, final_state, ob_sum, ob_sumsq, cluster, why, st);
+}
+
+int dne_launch_pendulum_binned_episodes(const dne_net_desc* net, const float* theta, const float* noise,
+                                        const int64_t* noise_idx, const float* scale, const int32_t* theta_idx,
+                                        int n_members, const double* init_state, int max_steps, const float* ob_mean,
+                                        const float* ob_std, const float* ac_noise, float* returns, float* signreturns,
+                                        int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq,
+                                        const float* bins, int nb, int cluster, const char** why, cudaStream_t st) {
+    return launch_binned<PendulumTask>(net, NoParams{}, bins, nb, theta, noise, noise_idx, scale, theta_idx, n_members,
+                                       init_state, max_steps, ob_mean, ob_std, ac_noise, returns, signreturns, lengths,
+                                       final_state, ob_sum, ob_sumsq, cluster, why, st);
+}
+
+int dne_launch_maze_binned_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta,
+                                    const float* noise, const int64_t* noise_idx, const float* scale,
+                                    const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
+                                    const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
+                                    float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
+                                    double* ob_sumsq, const float* bins, int nb, int cluster, const char** why,
+                                    cudaStream_t st) {
+    return launch_binned<MazeTask>(net, make_maze_params(maze), bins, nb, theta, noise, noise_idx, scale, theta_idx,
+                                   n_members, init_state, max_steps, ob_mean, ob_std, ac_noise, returns, signreturns,
+                                   lengths, final_state, ob_sum, ob_sumsq, cluster, why, st);
 }

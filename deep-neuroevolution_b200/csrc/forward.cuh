@@ -135,6 +135,24 @@ int dne_launch_maze_cluster_episodes(const dne_maze_desc* maze, const dne_net_de
                                      const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
                                      float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
                                      double* ob_sumsq, int cluster, const char** why, cudaStream_t st);
+// episode_kernels.cu: the same episodes with a discretised head of `nb` bins per action dimension (dne_*_binned_episodes);
+// `bins` is the host table [N_OUT][nb] (non-null, checked).  `cluster` 0 runs the single-CTA kernel when the member fits
+// one CTA and the automatic cluster size otherwise; 2, 4, 8 force the cluster kernel at that size.
+bool dne_pendulum_binned_net_supported(const dne_net_desc* net, int nb, const char** why);
+bool dne_maze_binned_net_supported(const dne_net_desc* net, int nb, const char** why);
+int dne_launch_pendulum_binned_episodes(const dne_net_desc* net, const float* theta, const float* noise,
+                                        const int64_t* noise_idx, const float* scale, const int32_t* theta_idx,
+                                        int n_members, const double* init_state, int max_steps, const float* ob_mean,
+                                        const float* ob_std, const float* ac_noise, float* returns, float* signreturns,
+                                        int32_t* lengths, double* final_state, double* ob_sum, double* ob_sumsq,
+                                        const float* bins, int nb, int cluster, const char** why, cudaStream_t st);
+int dne_launch_maze_binned_episodes(const dne_maze_desc* maze, const dne_net_desc* net, const float* theta,
+                                    const float* noise, const int64_t* noise_idx, const float* scale,
+                                    const int32_t* theta_idx, int n_members, const double* init_state, int max_steps,
+                                    const float* ob_mean, const float* ob_std, const float* ac_noise, float* returns,
+                                    float* signreturns, int32_t* lengths, double* final_state, double* ob_sum,
+                                    double* ob_sumsq, const float* bins, int nb, int cluster, const char** why,
+                                    cudaStream_t st);
 
 int dne_launch_theta_gemm_tc(const float* X, int M, int K, int N, const float* W, int k_per_split, int n_split,
                              float* part, cudaStream_t st);

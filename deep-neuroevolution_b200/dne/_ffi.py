@@ -77,6 +77,12 @@ _SIGS = {
                                   _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, _P],
     "dne_pendulum_cluster_geometry": [C.POINTER(NetDesc), C.c_int, C.POINTER(C.c_int)],
     "dne_maze_cluster_geometry": [C.POINTER(NetDesc), C.c_int, C.POINTER(C.c_int)],
+    "dne_pendulum_binned_net_supported": [C.POINTER(NetDesc), C.c_int],
+    "dne_maze_binned_net_supported": [C.POINTER(NetDesc), C.c_int],
+    "dne_pendulum_binned_episodes": [_P, C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P,
+                                     _P, _P, _P, _P, _P, C.c_int, C.c_int, _P],
+    "dne_maze_binned_episodes": [_P, C.POINTER(MazeDesc), C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P,
+                                 _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P],
     "dne_theta_prepare": [_P, C.POINTER(NetDesc), _P, C.c_int, _P, C.c_size_t, _P],
     "dne_theta_forget": [_P, _P],
     "dne_vbn_ws_bytes": [C.POINTER(NetDesc), C.c_int, C.c_int, C.POINTER(C.c_size_t)],

@@ -387,17 +387,28 @@ class PendulumEnv(BatchEnv):
         """float64 [k, 2] reset states (th, thdot)."""
         return self.rs.uniform(low=-self.HIGH, high=self.HIGH, size=(int(k), 2))
 
-    def episode_net_supported(self, net) -> bool:
+    def episode_net_supported(self, net, action_bins=None) -> bool:
+        """Whether ``dne_pendulum_episodes`` takes ``net`` (with ``action_bins``, the policy's [1, nb] bin table:
+        whether ``dne_pendulum_binned_episodes`` takes it, on one CTA or a cluster)."""
+        if action_bins is not None:
+            return F.lib().dne_pendulum_binned_net_supported(C.byref(net.desc), _bin_table(action_bins, 1).shape[1]) == 0
         return F.lib().dne_pendulum_net_supported(C.byref(net.desc)) == 0
 
     def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
-                        d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None):
+                        d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None,
+                        action_bins=None):
         """One member per CTA group (``dne_pendulum_episodes``) when the net fits a CTA, otherwise one member per
-        thread-block cluster (``dne_pendulum_cluster_episodes``, automatic size): the same numbers either way."""
+        thread-block cluster (``dne_pendulum_cluster_episodes``, automatic size): the same numbers either way.
+        ``action_bins``: the policy's float32 [1, nb] bin table of a discretised head, run by
+        ``dne_pendulum_binned_episodes`` (which picks the kernel the same way; ``d_ac_noise`` is then [n, limit, 1])."""
         args = (C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale), F.ptr(d_row), n,
                 F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise), F.ptr(d_ret),
                 F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq))
-        if self.episode_net_supported(net):
+        if action_bins is not None:
+            tab = _bin_table(action_bins, 1)
+            F.check(F.lib().dne_pendulum_binned_episodes(ctx.handle, *args, tab.ctypes.data_as(C.c_void_p),
+                                                         tab.shape[1], 0, F.stream_ptr()))
+        elif self.episode_net_supported(net):
             F.check(F.lib().dne_pendulum_episodes(ctx.handle, *args, F.stream_ptr()))
         else:
             F.check(F.lib().dne_pendulum_cluster_episodes(ctx.handle, *args, 0, F.stream_ptr()))
@@ -430,6 +441,14 @@ class PendulumEnv(BatchEnv):
 
     def random_actions(self, k, rs):
         return rs.uniform(-2.0, 2.0, size=(k, 1)).astype(np.float32)
+
+
+def _bin_table(action_bins, adim: int) -> np.ndarray:
+    """The policy's bin table as the binned entries take it: C-contiguous float32 [adim, nb]."""
+    tab = np.ascontiguousarray(action_bins, dtype=np.float32)
+    if tab.ndim != 2 or tab.shape[0] != adim:
+        raise ValueError(f"action_bins must be [{adim}, n_bins] (one row per action dimension), got {tab.shape}")
+    return tab
 
 
 def _make_pendulum(env_id, n_slots, seed=0, episode_len=None, **kw):
@@ -474,19 +493,26 @@ class MazeEnv(BatchEnv):
         s[:, 0], s[:, 1] = self.start
         return s
 
-    def episode_net_supported(self, net) -> bool:
+    def episode_net_supported(self, net, action_bins=None) -> bool:
         return True                # the only path: the kernel itself rejects a net it cannot run
 
     def launch_episodes(self, ctx, net, theta, d_idx, d_scale, d_row, n, d_init, limit, d_ret, d_sret, d_len, d_fin,
-                        d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None):
+                        d_ob_mean=None, d_ob_std=None, d_ac_noise=None, d_ob_sum=None, d_ob_sumsq=None,
+                        action_bins=None):
         """One member per CTA group (``dne_maze_episodes``) when the net fits a CTA, otherwise one member per
         thread-block cluster (``dne_maze_cluster_episodes``, automatic size; MujocoPolicy's hidden [256, 256]): the same
-        numbers either way.  A net neither kernel takes raises with the cluster entry's reason."""
+        numbers either way.  A net neither kernel takes raises with the cluster entry's reason.  ``action_bins``: the
+        policy's float32 [2, nb] bin table of a discretised head, run by ``dne_maze_binned_episodes`` (which picks the
+        kernel the same way; ``d_ac_noise`` is then [n, limit, 2])."""
         L = F.lib()
         args = (C.byref(self.desc), C.byref(net.desc), F.ptr(theta, torch.float32), F.ptr(d_idx), F.ptr(d_scale),
                 F.ptr(d_row), n, F.ptr(d_init), int(limit), F.ptr(d_ob_mean), F.ptr(d_ob_std), F.ptr(d_ac_noise),
                 F.ptr(d_ret), F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_ob_sum), F.ptr(d_ob_sumsq))
-        if L.dne_maze_net_supported(C.byref(net.desc)) == 0:
+        if action_bins is not None:
+            tab = _bin_table(action_bins, 2)
+            F.check(L.dne_maze_binned_episodes(ctx.handle, *args, tab.ctypes.data_as(C.c_void_p), tab.shape[1], 0,
+                                               F.stream_ptr()))
+        elif L.dne_maze_net_supported(C.byref(net.desc)) == 0:
             F.check(L.dne_maze_episodes(ctx.handle, *args, F.stream_ptr()))
         else:
             F.check(L.dne_maze_cluster_episodes(ctx.handle, *args, 0, F.stream_ptr()))

@@ -261,10 +261,15 @@ class EpisodeKernelRunner:
     ``env.initial_states(n_units*G)`` call per ``run``.  When the environment's kernel takes MujocoPolicy's inputs
     (``env.kernel_policy_io``), ``run`` also draws, from ``random_stream``: first one ``rand()`` per non-noiseless member in
     (unit, member) order against ``save_obs_prob`` (the members whose observations go into the statistics), then one
-    ``randn(n_noisy, limit, 1)`` of action noise for the non-noiseless members, scaled as ``RolloutRunner`` scales it."""
+    ``randn(n_noisy, limit, adim)`` of action noise for the non-noiseless members, scaled as ``RolloutRunner`` scales it
+    (adim: the action dimensions, ``net.n_out`` for a linear head).
+
+    ``action_bins``: MujocoPolicy's float32 [adim, nb] bin table of a discretised head ('uniform:' / 'custom:'); the kernel
+    then takes per dimension the bin of the highest score (numpy's argmax) and acts with its value, as ``action_fn``
+    followed by ``RolloutRunner``'s noise would."""
 
     def __init__(self, ctx: F.Context, net: NetSpec, env: BatchEnv, n_slots: int = 0, group: int = 2, pipeline: int = 1,
-                 ref_batch: Optional[torch.Tensor] = None):
+                 ref_batch: Optional[torch.Tensor] = None, action_bins=None):
         assert getattr(env, "device_episodes", False), "EpisodeKernelRunner needs an environment with device episodes"
         if net.needs_ref_batch:
             raise NotImplementedError("the episode kernel runs nets without batch norm only")
@@ -273,6 +278,14 @@ class EpisodeKernelRunner:
         self.halves = (None,)          # one launch covers every member (drivers read len(halves) as tables per launch)
         self.use_theta_idx = False
         self.action_fn = None          # accepted for interface parity; the kernel's head is the environment's action
+        self.action_bins = None
+        if action_bins is not None:
+            if not env.kernel_policy_io:
+                raise NotImplementedError(f"{type(env).__name__}'s episode kernel has no discretised heads")
+            tab = np.ascontiguousarray(action_bins, dtype=np.float32)
+            if tab.ndim != 2 or tab.shape[0] * tab.shape[1] != net.n_out:
+                raise ValueError(f"action_bins {tab.shape} do not match the net's {net.n_out} outputs (adim * n_bins)")
+            self.action_bins = tab
 
     def run(self, theta: torch.Tensor, units: List[Unit], timestep_limit: Optional[int] = None, *, ob_mean=None,
             ob_std=None, collect_bc: Optional[str] = None, ac_noise_std: float = 0.0,
@@ -317,10 +330,13 @@ class EpisodeKernelRunner:
                 extra["d_ob_sum"] = torch.empty(n, self.net.ob_dim, dtype=torch.float64, device=dev)
                 extra["d_ob_sumsq"] = torch.empty_like(extra["d_ob_sum"])
             if ac_noise_std != 0.0 and random_stream is not None:          # policies.py:204-205, RolloutRunner.finish
-                ac = np.zeros((n, int(limit), self.net.n_out), dtype=np.float32)
-                ac[noisy] = random_stream.randn(int(noisy.sum()), int(limit), self.net.n_out).astype(np.float32) * \
+                adim = self.net.n_out if self.action_bins is None else self.action_bins.shape[0]
+                ac = np.zeros((n, int(limit), adim), dtype=np.float32)
+                ac[noisy] = random_stream.randn(int(noisy.sum()), int(limit), adim).astype(np.float32) * \
                     np.float32(ac_noise_std)
                 extra["d_ac_noise"] = torch.from_numpy(ac).to(dev)
+            if self.action_bins is not None:
+                extra["action_bins"] = self.action_bins
             if ob_mean is not None:
                 extra["d_ob_mean"] = ob_mean.to(dev, torch.float32).contiguous()
                 extra["d_ob_std"] = ob_std.to(dev, torch.float32).contiguous()
@@ -363,16 +379,27 @@ class EpisodeKernelRunner:
         return res
 
 
-def make_runner(ctx: F.Context, net: NetSpec, env: BatchEnv, action_fn=None, **kw):
+def make_runner(ctx: F.Context, net: NetSpec, env: BatchEnv, action_fn=None, action_bins=None, **kw):
     """The rollout runner for ``env``: ``EpisodeKernelRunner`` when its episodes run on the device
     (``env.device_episodes``), the environment's kernel takes ``net`` (``env.episode_net_supported``) and no host
     ``action_fn`` maps the network's output to actions; otherwise the per-tick ``RolloutRunner`` when the environment
     has a host step.  ``action_fn``: the policy's map from output rows to actions (discretised MuJoCo heads), None for
-    the identity; an environment without a host step refuses one.  ``kw`` are ``RolloutRunner``'s arguments."""
+    the identity; an environment without a host step refuses one unless ``action_bins`` comes with it.
+    ``action_bins``: the bin table [adim, nb] behind a discretised ``action_fn`` (MujocoPolicy's ``_bin_values``); an
+    environment without a host step (the maze) then runs the head in its episode kernel (``EpisodeKernelRunner``), one
+    with a host step keeps the per-tick runner with ``action_fn``.  ``kw`` are ``RolloutRunner``'s arguments."""
     device = getattr(env, "device_episodes", False)
+    if action_bins is not None:
+        if action_fn is None:
+            raise ValueError("action_bins comes with the policy's action_fn (the host map of the same head)")
+        if device and not env.host_step:
+            r = EpisodeKernelRunner(ctx, net, env, action_bins=action_bins, **kw)
+            r.action_fn = action_fn
+            return r
     if device and action_fn is not None and not env.host_step:
         raise NotImplementedError(f"{type(env).__name__} runs only on its episode kernel, whose head is the action: a "
-                                  "discretised ('uniform:' / 'custom:') head needs a host action map; use 'continuous:'")
+                                  "discretised ('uniform:' / 'custom:') head runs there only with its bin table "
+                                  "(action_bins); otherwise use 'continuous:'")
     if device and ((action_fn is None and env.episode_net_supported(net)) or not env.host_step):
         r = EpisodeKernelRunner(ctx, net, env, **kw)
     else:

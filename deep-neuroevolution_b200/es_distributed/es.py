@@ -349,8 +349,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     vine = bool(exp.get('vine_export'))        # es_modified.py: per-generation BC point clouds for the visual inspector
     group = 2
     runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=group,
-                         pipeline=2 if n_slots % 4 == 0 else 1, ref_batch=policy.ref_batch,
-                         action_fn=policy.action_fn if getattr(policy, "_bin_values", None) is not None else None)
+                         pipeline=2 if n_slots % 4 == 0 else 1, ref_batch=policy.ref_batch, **policy.runner_head_kw())
 
     episodes_so_far = timesteps_so_far = 0
     tstart = time.time()

@@ -101,7 +101,8 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     elite = None
     deep_stats, deep_extra = {}, {}
     cache = GenomeCache(ctx, policy.net, config.noise_stdev, exp.get('ga_mode', 'cpu'))
-    runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1)
+    runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=1, pipeline=2 if n_slots % 2 == 0 else 1,
+                         **policy.runner_head_kw())
     ob_stat = dict(ob_mean=policy.ob_mean, ob_std=policy.ob_std)            # MujocoPolicy: its fixed statistics
     population, population_score = [], np.array([], dtype=np.float32)
     episodes_so_far = timesteps_so_far = 0

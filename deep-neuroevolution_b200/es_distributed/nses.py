@@ -133,8 +133,7 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
     if policy.needs_ref_batch:
         policy.set_ref_batch(get_ref_batch(env, batch_size=128, rs=np.random.RandomState(seed)))
     runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=2, pipeline=2 if n_slots % 4 == 0 else 1,
-                         ref_batch=policy.ref_batch,
-                         action_fn=policy.action_fn if getattr(policy, "_bin_values", None) is not None else None)
+                         ref_batch=policy.ref_batch, **policy.runner_head_kw())
     # behaviour characterisation per policy family: RAM trace for the Atari policies (policies.py:410,418), final (x, y)
     # position for MujocoPolicy (policies.py:292-299, bc_choice default)
     vector_bc = policy.net.ob_kind == F.OB_VECTOR

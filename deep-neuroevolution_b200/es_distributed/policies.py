@@ -214,10 +214,18 @@ class Policy:
     def act(self, ob, random_stream=None):
         raise NotImplementedError
 
+    def runner_head_kw(self) -> dict:
+        """``make_runner``'s head arguments for this policy: for MujocoPolicy's discretised heads the host map from
+        scores to bin values (``action_fn``) and its bin table (``action_bins``, for the episode kernels); nothing for a
+        head whose output is the action."""
+        bins = getattr(self, "_bin_values", None)
+        return {} if bins is None else {"action_fn": self.action_fn, "action_bins": bins}
+
     def rollout(self, env, *, render=False, timestep_limit=None, save_obs=False, random_stream=None, **_):
         """policies.py:71-97 -- one episode of the CURRENT weights on slot 0 of a ``dne.envs.BatchEnv``.
         Returns (rews_sum_as_array, t, novelty_vector) like the Atari variants (policies.py:429,513)."""
-        runner = make_runner(self._ctx, self.net, env, n_slots=2, group=1, pipeline=1, ref_batch=self.ref_batch)
+        runner = make_runner(self._ctx, self.net, env, n_slots=2, group=1, pipeline=1, ref_batch=self.ref_batch,
+                             **self.runner_head_kw())
         res = runner.run(self._theta, [Unit(0, (0.0,))], timestep_limit, ob_mean=self.ob_mean, ob_std=self.ob_std,
                          collect_bc="final", ac_noise_std=getattr(self, "ac_noise_std", 0.0), random_stream=random_stream)
         return np.array([res.returns[0, 0]], dtype=np.float32), int(res.lengths[0, 0]), res.bcs[0][0]

@@ -283,6 +283,36 @@ int dne_maze_cluster_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne
 int dne_pendulum_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry);
 int dne_maze_cluster_geometry(const dne_net_desc* net, int cluster, int* geometry);
 
+/* Pendulum-v1 and hard-maze episodes for MujocoPolicy's discretised heads ('uniform:N', 'custom:v0,..,vk'; DESIGN.md
+ * 3.9), with adim = 1 (Pendulum) or 2 (maze) action dimensions of n_bins bins each.  Arguments, outputs and numerics as
+ * dne_*_cluster_episodes, plus bin_values_host, the policy's float32 table [adim][n_bins] on the HOST (copied into the
+ * launch), and n_bins.  Per step the net's n_out = adim * n_bins outputs are scores, each a sequential fmaf over its
+ * inputs in index order, then + bias; score d * n_bins + b is bin b of action dimension d.  For each dimension the bin
+ * taken is the first one whose score is NaN if any is, otherwise the first maximum (numpy's argmax); the action is
+ * a[d] = bin_values_host[d][bin], then + d_ac_noise[m][step][d] (nullable [n][max_steps][adim]: the noise is added after
+ * the discretisation, and has adim, not n_out, components).  The task's step (Pendulum's clip, the maze's rate limits),
+ * the observation normalisation and sums, returns, sign-returns and final states are the continuous entries'.
+ * cluster 0 runs one member per CTA group when it fits one CTA and otherwise picks the cluster size as
+ * dne_*_cluster_episodes does; 2, 4 or 8 force a cluster of that size (the outputs are bit-identical either way);
+ * anything else returns DNE_ERR_ARG.  A NULL bin_values_host returns DNE_ERR_ARG.  Supported: 2 <= n_bins <= 32,
+ * n_out = adim * n_bins, and otherwise the nets dne_*_cluster_net_supported takes; anything else returns DNE_ERR_UNSUP
+ * with the reason in dne_last_error().  dne_*_binned_net_supported answers the same question without launching (0 or
+ * DNE_ERR_UNSUP).  The continuous entries above are unchanged and still refuse n_out != adim. */
+int dne_pendulum_binned_net_supported(const dne_net_desc* net, int n_bins);
+int dne_maze_binned_net_supported(const dne_net_desc* net, int n_bins);
+int dne_pendulum_binned_episodes(dne_ctx* ctx, const dne_net_desc* net, const float* d_theta,
+                                 const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx,
+                                 int n_members, const double* d_init_state, int max_steps, const float* d_ob_mean,
+                                 const float* d_ob_std, const float* d_ac_noise, float* d_returns, float* d_signreturns,
+                                 int32_t* d_lengths, double* d_final_state, double* d_ob_sum, double* d_ob_sumsq,
+                                 const float* bin_values_host, int n_bins, int cluster, void* stream);
+int dne_maze_binned_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_net_desc* net, const float* d_theta,
+                             const int64_t* d_noise_idx, const float* d_scale, const int32_t* d_theta_idx, int n_members,
+                             const double* d_init_state, int max_steps, const float* d_ob_mean, const float* d_ob_std,
+                             const float* d_ac_noise, float* d_returns, float* d_signreturns, int32_t* d_lengths,
+                             double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, const float* bin_values_host,
+                             int n_bins, int cluster, void* stream);
+
 /* Observation statistics of the running normaliser (es.py:356-363 rollout_and_update_ob_stat; RunningStat es.py:26-48):
  * adds the observations d_obs[slot, :] (float32 [*, ob_dim], the unnormalised vectors fed to this tick's forward) of the m
  * listed slots -- the slots whose episode was sampled with probability calc_obstat_prob -- into float64 running sums

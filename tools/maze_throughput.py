@@ -1,6 +1,7 @@
 """Hard-maze throughput of the continuous episode kernel (needs an H100).
 
-    python tools/maze_throughput.py [--launches 20] [--gens 10] [--hidden 256 256] [--cluster {0,2,4,8}] [--out FILE.json]
+    python tools/maze_throughput.py [--launches 20] [--gens 10] [--hidden 256 256] [--cluster {0,2,4,8}]
+                                    [--ac-bins uniform:10] [--out FILE.json]
 
 Reports, from one process, for configurations/hardmaze_nses.json (MujocoPolicy, 400-step episodes; --hidden replaces its
 hidden_dims, e.g. the reference's humanoid [256, 256]):
@@ -13,6 +14,8 @@ hidden_dims, e.g. the reference's humanoid [256, 256]):
 The kernel is dne_maze_episodes when the net fits one CTA, otherwise dne_maze_cluster_episodes at the automatic cluster
 size, as MazeEnv launches it; --cluster forces the cluster entry at that size (0: automatic), and the result then also
 reports its geometry (cluster size, threads and shared bytes per CTA, resident members).  --gens 0 skips the generation.
+--ac-bins (a MujocoPolicy head, e.g. uniform:10 or custom:-1,0,1) also times dne_maze_binned_episodes for the same
+hidden sizes and members (binned_kernel_*), beside the continuous kernel; the generation then runs with that head.
 """
 import argparse
 import ctypes as C
@@ -43,7 +46,7 @@ def card():
     return {"name": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip() or q.stderr.strip()}
 
 
-def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
+def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None, bins=None):
     dev = torch.device("cuda", 0)
     rs = np.random.RandomState(seed)
     P = net.num_params
@@ -64,11 +67,16 @@ def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
     args = (C.byref(env.desc), C.byref(net.desc), F.ptr(th), F.ptr(d_idx), F.ptr(d_sc), None, n, F.ptr(d_init), T,
             F.ptr(d_mean), F.ptr(d_std), F.ptr(d_ac), F.ptr(d_ret), F.ptr(d_sret), F.ptr(d_len), F.ptr(d_fin), F.ptr(d_s),
             F.ptr(d_q))
-    if cluster is None and F.lib().dne_maze_net_supported(C.byref(net.desc)) != 0:
+    if bins is not None:
+        tab = np.ascontiguousarray(bins, dtype=np.float32)
+    elif cluster is None and F.lib().dne_maze_net_supported(C.byref(net.desc)) != 0:
         cluster = 0                                   # MazeEnv's choice for a net too wide for one CTA
 
     def launch():
-        if cluster is None:
+        if bins is not None:                          # one CTA when the member fits one, as MazeEnv launches it
+            F.check(F.lib().dne_maze_binned_episodes(ctx.handle, *args, tab.ctypes.data_as(C.c_void_p), tab.shape[1],
+                                                     cluster or 0, F.stream_ptr()))
+        elif cluster is None:
             F.check(F.lib().dne_maze_episodes(ctx.handle, *args, F.stream_ptr()))
         else:
             F.check(F.lib().dne_maze_cluster_episodes(ctx.handle, *args, cluster, F.stream_ptr()))
@@ -83,7 +91,7 @@ def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / launches
     res = {"members": n, "launches": launches, "kernel_ms": ms, "env_steps_per_s": n * T / (ms * 1e-3)}
-    if cluster is not None:
+    if cluster is not None and bins is None:
         res["cluster_geometry"] = F.cluster_geometry("maze", net.desc, cluster)
     return res
 
@@ -95,6 +103,7 @@ def main():
     ap.add_argument("--hidden", type=int, nargs="+", default=None, help="hidden_dims instead of the config's")
     ap.add_argument("--cluster", type=int, choices=(0, 2, 4, 8), default=None,
                     help="force dne_maze_cluster_episodes at this cluster size (0: automatic)")
+    ap.add_argument("--ac-bins", default=None, help="also time this discretised head (e.g. uniform:10)")
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
@@ -111,6 +120,13 @@ def main():
     out["kernel_config_population"] = time_kernel(ctx, pol.net, pol.device_theta, exp["config"]["episodes_per_batch"],
                                                   args.launches, cluster=args.cluster)
     out["kernel_5000"] = time_kernel(ctx, pol.net, pol.device_theta, 5000, args.launches, cluster=args.cluster)
+    if args.ac_bins:
+        exp["policy"]["args"]["ac_bins"] = out["ac_bins"] = args.ac_bins
+        bp = policies.MujocoPolicy(env.observation_space, env.action_space, seed=0, **exp["policy"]["args"])
+        for key, n in (("binned_kernel_config_population", exp["config"]["episodes_per_batch"]),
+                       ("binned_kernel_5000", 5000)):
+            out[key] = time_kernel(ctx, bp.net, bp.device_theta, n, args.launches, cluster=args.cluster,
+                                   bins=bp._bin_values)
     if args.gens > 0:
         gens = []
         NS.run_master(None, None, exp, max_iterations=args.gens, seed=0,

@@ -1,7 +1,7 @@
 """Pendulum-v1 throughput of the fused episode kernel (needs an H100).
 
     python tools/pendulum_throughput.py [--launches 50] [--gens 10] [--per-tick-members 256] [--hidden 256 256]
-                                        [--cluster {0,2,4,8}] [--out FILE.json]
+                                        [--cluster {0,2,4,8}] [--ac-bins uniform:5] [--out FILE.json]
 
 Reports, from one process, for configurations/pendulum_es.json (MujocoPolicy, 200-step episodes; --hidden replaces its
 hidden_dims, e.g. the reference's humanoid [256, 256]):
@@ -18,6 +18,9 @@ The kernel is dne_pendulum_episodes when the net fits one CTA, otherwise dne_pen
 cluster size, as PendulumEnv launches it; --cluster forces the cluster entry at that size (0: automatic), and the kernel
 results then also report its geometry (cluster size, threads and shared bytes per CTA, resident members).  --gens 0
 skips the generation and the runner costs, --per-tick-members 0 the per-tick comparison.
+--ac-bins (a MujocoPolicy head, e.g. uniform:5) also times dne_pendulum_binned_episodes for the same hidden sizes and
+members (binned_kernel_*), beside the continuous kernel, and the per-tick RolloutRunner with the policy's host action_fn
+against EpisodeKernelRunner(action_bins=...) (binned_per_tick_vs_kernel).
 """
 import argparse
 import ctypes as C
@@ -48,7 +51,7 @@ def card():
     return {"name": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip() or q.stderr.strip()}
 
 
-def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
+def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None, bins=None):
     dev = torch.device("cuda", 0)
     rs = np.random.RandomState(seed)
     P, T = net.num_params, 200
@@ -66,11 +69,16 @@ def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
 
     args = (C.byref(net.desc), F.ptr(th), F.ptr(d_idx), F.ptr(d_sc), None, n, F.ptr(d_init), T, F.ptr(d_mean),
             F.ptr(d_std), F.ptr(d_ac), F.ptr(d_ret), F.ptr(d_sret), F.ptr(d_len), None, F.ptr(d_s), F.ptr(d_q))
-    if cluster is None and F.lib().dne_pendulum_net_supported(C.byref(net.desc)) != 0:
+    if bins is not None:
+        tab = np.ascontiguousarray(bins, dtype=np.float32)
+    elif cluster is None and F.lib().dne_pendulum_net_supported(C.byref(net.desc)) != 0:
         cluster = 0                                   # PendulumEnv's choice for a net too wide for one CTA
 
     def launch():
-        if cluster is None:
+        if bins is not None:                          # one CTA when the member fits one, as PendulumEnv launches it
+            F.check(F.lib().dne_pendulum_binned_episodes(ctx.handle, *args, tab.ctypes.data_as(C.c_void_p),
+                                                         tab.shape[1], cluster or 0, F.stream_ptr()))
+        elif cluster is None:
             F.check(F.lib().dne_pendulum_episodes(ctx.handle, *args, F.stream_ptr()))
         else:
             F.check(F.lib().dne_pendulum_cluster_episodes(ctx.handle, *args, cluster, F.stream_ptr()))
@@ -85,17 +93,20 @@ def time_kernel(ctx, net, theta, n, launches, seed=0, cluster=None):
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / launches
     res = {"members": n, "launches": launches, "kernel_ms": ms, "env_steps_per_s": n * T / (ms * 1e-3)}
-    if cluster is not None:
+    if cluster is not None and bins is None:
         res["cluster_geometry"] = F.cluster_geometry("pendulum", net.desc, cluster)
     return res
 
 
-def per_tick_vs_kernel(ctx, net, theta, n, rounds=3):
+def per_tick_vs_kernel(ctx, net, theta, n, rounds=3, pol=None):
+    """pol: a discretised-head policy, whose bins the kernel runner takes and whose action_fn the per-tick one."""
     rs = np.random.RandomState(1)
     units = [Unit(int(rs.randint(0, ES.default_noise().count - net.num_params)), (0.02, -0.02)) for _ in range(n // 2)]
     mean, std = torch.zeros(3, device="cuda"), torch.tensor([0.7, 0.7, 3.0], device="cuda")
-    runners = {"kernel": EpisodeKernelRunner(ctx, net, PendulumEnv(n, seed=2), group=2),
+    runners = {"kernel": EpisodeKernelRunner(ctx, net, PendulumEnv(n, seed=2), group=2,
+                                             action_bins=None if pol is None else pol._bin_values),
                "per_tick": RolloutRunner(ctx, net, PendulumEnv(n, seed=2), n, group=2, pipeline=2)}
+    runners["per_tick"].action_fn = None if pol is None else pol.action_fn
     out = {k: [] for k in runners}
     for name, r in runners.items():                     # warm-up
         r.run(theta, units, None, ob_mean=mean, ob_std=std)
@@ -142,6 +153,7 @@ def main():
     ap.add_argument("--hidden", type=int, nargs="+", default=None, help="hidden_dims instead of the config's")
     ap.add_argument("--cluster", type=int, choices=(0, 2, 4, 8), default=None,
                     help="force dne_pendulum_cluster_episodes at this cluster size (0: automatic) in the kernel timings")
+    ap.add_argument("--ac-bins", default=None, help="also time this discretised head (e.g. uniform:5)")
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
@@ -168,6 +180,16 @@ def main():
         out["runner_costs"] = runner_costs(ctx, pol.net, pol.device_theta, cfg["episodes_per_batch"] // 2)
     if args.per_tick_members > 0:
         out["per_tick_vs_kernel"] = per_tick_vs_kernel(ctx, pol.net, pol.device_theta, args.per_tick_members)
+    if args.ac_bins:
+        out["ac_bins"] = args.ac_bins
+        bp = policies.MujocoPolicy(env.observation_space, env.action_space, seed=0,
+                                   **dict(exp["policy"]["args"], ac_bins=args.ac_bins))
+        for key, n in (("binned_kernel_config_population", n_cfg), ("binned_kernel_5000", 5000)):
+            out[key] = time_kernel(ctx, bp.net, bp.device_theta, n, args.launches, cluster=args.cluster,
+                                   bins=bp._bin_values)
+        if args.per_tick_members > 0:
+            out["binned_per_tick_vs_kernel"] = per_tick_vs_kernel(ctx, bp.net, bp.device_theta, args.per_tick_members,
+                                                                  pol=bp)
     out["card_after"] = card()
     print(json.dumps(out, indent=1))
     if args.out:

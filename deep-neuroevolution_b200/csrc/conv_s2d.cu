@@ -141,6 +141,64 @@ __device__ __forceinline__ void store_split_pair(uint4* p_hi, uint4* p_lo, int w
     reinterpret_cast<uint32_t*>(p_lo)[word] = lo;
 }
 
+// The fused epilogue of one member: registers -> (/255) + bias (+BN) + activation -> global (NHWC floats + Xc, or the next
+// layer's image).  It is straight-line code (the accumulators are registers) that runs once per member, so every
+// instruction on its path is fetched cold, and that fetch, not the stores, sets its time.  The variants keep the
+// per-value path short: MODE 0 = NHWC, 1 / 2 = next image with space-to-depth stride 1 / 2 (the divisions by the stride
+// fold away), -1 = any (read from so); FAST = no batch norm and ReLU (no branch per value).  Every variant computes each
+// value with the same operations in the same order.
+template <int COUT, int HOUT, int W, int MT, int NTW, int ACC, bool IN_U8, int MODE, bool FAST>
+__device__ __forceinline__ void s2d_epilogue(const float (&acc)[NTW][ACC], const float (&cor)[NTW][ACC], int w, int wq, int lane,
+                                             const float* sb, const float* sm, const float* si, const float* sg, const float* se,
+                                             int act, bool bn, const S2dOut& so, float* outp, int slot) {
+    constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
+    const bool next_img = MODE < 0 ? so.next_img != 0 : MODE > 0;
+    const int nS = MODE > 0 ? MODE : so.nS;
+#pragma unroll
+    for (int j = 0; j < NTW; ++j) {
+        const int t = w + 2 * j;
+        if (t >= MT) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = t * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            const int oy = m / W, ox = m - oy * W;
+            if (oy >= HOUT || ox >= HOUT) continue;
+#pragma unroll
+            for (int i = 0; i < COUT / 8; ++i) {
+                const int n = 8 * i + 2 * (lane & 3);
+                float v[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float r = fmaf(cor[j][4 * i + 2 * h + e], F16_LO_INV, acc[j][4 * i + 2 * h + e]);   // main + 2^-11 * correction
+                    if (IN_U8) r *= IN_SCALE;
+                    r += sb[n + e];
+                    if (FAST) {
+                        v[e] = fmaxf(r, 0.0f);
+                    } else {
+                        if (bn) r = (r - sm[n + e]) * si[n + e] * sg[n + e] + se[n + e];   // policies.py:322
+                        v[e] = act == DNE_ACT_RELU ? fmaxf(r, 0.0f) : (act == DNE_ACT_TANH ? tanhf(r) : r);
+                    }
+                }
+                if (!next_img) {
+                    *reinterpret_cast<float2*>(outp + (int64_t)(oy * HOUT + ox) * COUT + n) = make_float2(v[0], v[1]);
+                    if (so.xc) {
+                        const int ko = ((oy * HOUT + ox) * COUT + 8 * i) >> 3;
+                        uint4* xp = reinterpret_cast<uint4*>(so.xc) + ((int64_t)(slot >> 7) * so.xc_ko + ko) * 256 + (slot & 127);
+                        store_split_pair(xp, xp + 128, lane & 3, v[0], v[1]);
+                    }
+                } else {
+                    const int Y = oy + so.nPADB, X = ox + so.nPADB;
+                    const int pix = (Y / nS) * so.nW + (X / nS);
+                    const int pp = (Y % nS) * nS + (X % nS);
+                    const int co = pp * (COUT / 8) + i;                             // channel octet of the next image
+                    uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
+                    store_split_pair(p, p + (size_t)2 * so.nPIXP, lane & 3, v[0], v[1]);
+                }
+            }
+        }
+    }
+}
+
 template <int CIN, int COUT, int KS, int S, int HIN, int HOUT, int PAD, bool IN_U8>
 __global__ void __launch_bounds__(S2D_THREADS, 1)
 conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict__ in_base, int64_t in_slot_stride,
@@ -189,7 +247,6 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
         // ============ MMA warpgroups: wgmma into registers, then the fused epilogue of the member ============
         const int w = warp >> 2, wq = warp & 3;
         const int et = tid;                                      // 0 .. 255
-        constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
         const int act = epi.act;
         const bool bn = epi.bn != DNE_BN_NONE;
         // main and correction accumulators are separate register blocks: a wgmma into a sub-block of another wgmma's
@@ -268,44 +325,20 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
             mbar_arrive(&a_empty[NG - 1]);
             named_bar_sync(2, S2D_MMA_THREADS);                  // per-channel parameters (and padding) of this member ready
             // ---- epilogue: registers -> (/255) + bias (+BN) + activation -> global ----
-#pragma unroll
-            for (int j = 0; j < NTW; ++j) {
-                const int t = w + 2 * j;
-                if (t >= MT) continue;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int m = t * 64 + wq * 16 + (lane >> 2) + 8 * h;
-                    const int oy = m / W, ox = m - oy * W;
-                    if (oy >= HOUT || ox >= HOUT) continue;
-#pragma unroll
-                    for (int i = 0; i < COUT / 8; ++i) {
-                        const int n = 8 * i + 2 * (lane & 3);
-                        float v[2];
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            float r = fmaf(cor[j][4 * i + 2 * h + e], F16_LO_INV, acc[j][4 * i + 2 * h + e]);   // main + 2^-11 * correction
-                            if (IN_U8) r *= IN_SCALE;
-                            r += s_bias[pb][n + e];
-                            if (bn) r = (r - s_mean[pb][n + e]) * s_inv[pb][n + e] * s_gamma[pb][n + e] + s_beta[pb][n + e];   // policies.py:322
-                            v[e] = act == DNE_ACT_RELU ? fmaxf(r, 0.0f) : (act == DNE_ACT_TANH ? tanhf(r) : r);
-                        }
-                        if (!so.next_img) {
-                            *reinterpret_cast<float2*>(outp + (int64_t)(oy * HOUT + ox) * COUT + n) = make_float2(v[0], v[1]);
-                            if (so.xc) {
-                                const int ko = ((oy * HOUT + ox) * COUT + 8 * i) >> 3;
-                                uint4* xp = reinterpret_cast<uint4*>(so.xc) + ((int64_t)(slot >> 7) * so.xc_ko + ko) * 256 + (slot & 127);
-                                store_split_pair(xp, xp + 128, lane & 3, v[0], v[1]);
-                            }
-                        } else {
-                            const int Y = oy + so.nPADB, X = ox + so.nPADB;
-                            const int pix = (Y / so.nS) * so.nW + (X / so.nS);
-                            const int pp = (Y % so.nS) * so.nS + (X % so.nS);
-                            const int co = pp * (COUT / 8) + i;                             // channel octet of the next image
-                            uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
-                            store_split_pair(p, p + (size_t)2 * so.nPIXP, lane & 3, v[0], v[1]);
-                        }
-                    }
-                }
+            {
+                const float *sb = s_bias[pb], *sm = s_mean[pb], *si = s_inv[pb], *sg = s_gamma[pb], *se = s_beta[pb];
+                const bool relu_only = !bn && act == DNE_ACT_RELU;
+#define S2D_EPI(MODE, FAST)                                                                                              \
+    s2d_epilogue<COUT, HOUT, W, MT, NTW, Cfg::ACC, IN_U8, MODE, FAST>(acc, cor, w, wq, lane, sb, sm, si, sg, se, act, bn, so, \
+                                                                       outp, slot)
+                // the fast variant writes what follows this shape in the compiled nets (the shape list below): 32 -> 64
+                // channels -> a stride-1 image, the others -> NHWC.  The first layer keeps the generic one: its 128
+                // accumulator registers leave no room for a second copy (ptxas spills them).
+                constexpr int FAST_MODE = CIN == 32 ? 1 : 0;
+                if (!IN_U8 && relu_only && (FAST_MODE == 0 ? !so.next_img : (so.next_img && so.nS == FAST_MODE)))
+                    S2D_EPI(FAST_MODE, true);
+                else S2D_EPI(-1, false);
+#undef S2D_EPI
             }
             ++it;
         }

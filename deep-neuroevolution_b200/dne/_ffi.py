@@ -36,6 +36,7 @@ class NetDesc(C.Structure):
 
 
 MAZE_MAX_WALLS = 64
+IMAGE_MAZE_MAX_ACTIONS = 32
 
 
 class MazeDesc(C.Structure):
@@ -83,6 +84,9 @@ _SIGS = {
                                      _P, _P, _P, _P, _P, C.c_int, C.c_int, _P],
     "dne_maze_binned_episodes": [_P, C.POINTER(MazeDesc), C.POINTER(NetDesc), _P, _P, _P, _P, C.c_int, _P, C.c_int, _P,
                                  _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P],
+    "dne_image_maze_background": [C.POINTER(MazeDesc), _P, _P],
+    "dne_image_maze_reset": [C.POINTER(MazeDesc), _P, _P, _P, C.c_int, _P, _P, _P],
+    "dne_image_maze_step": [C.POINTER(MazeDesc), _P, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, _P, _P],
     "dne_theta_prepare": [_P, C.POINTER(NetDesc), _P, C.c_int, _P, C.c_size_t, _P],
     "dne_theta_forget": [_P, _P],
     "dne_vbn_ws_bytes": [C.POINTER(NetDesc), C.c_int, C.c_int, C.POINTER(C.c_size_t)],

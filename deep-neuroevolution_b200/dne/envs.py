@@ -11,7 +11,9 @@ here is the synthetic Frostbite-shaped stub the measurement plan names (SURVEY.m
 observations from a fixed pool, rewards 10*Bernoulli(0.05), fixed or ragged episode lengths.  A real emulator
 plugs in by subclassing ``BatchEnv``.  Four real tasks need no emulator: CartPole-v1 (``CartPoleEnv``), Acrobot-v1
 (``AcrobotEnv``), MountainCar-v0 (``MountainCarEnv``), Pendulum-v1 (``PendulumEnv``) and the reference's hard maze
-(``MazeEnv``), whose episodes run whole on the device (``dne.rollout.EpisodeKernelRunner``).
+(``MazeEnv``), whose episodes run whole on the device (``dne.rollout.EpisodeKernelRunner``).  The same maze seen as an
+84x84 image (``ImageMazeEnv``, ``ImageHardMaze-v0``) is the conv policies' real task: stepped and rendered on the device
+one tick at a time under the per-tick runner.
 
 An environment with device episodes (``device_episodes = True``) supplies ``state_dim``, ``initial_states(k)``,
 ``episode_net_supported(net)`` and ``launch_episodes(...)``; ``kernel_policy_io`` says whether its kernel also takes
@@ -481,11 +483,7 @@ class MazeEnv(BatchEnv):
         self.observation_space = Box(-np.inf, np.inf, (11,))
         self.action_space = Box(-0.5, 0.5, (2,))
         self.max_episode_steps = self.MAX_STEPS
-        self.desc = F.MazeDesc(n_walls=len(self.walls), collisions_stick=int(self.collisions_stick))
-        self.desc.goal[0], self.desc.goal[1] = self.goal
-        for j, w in enumerate(self.walls):
-            for k in range(4):
-                self.desc.walls[j][k] = float(w[k])
+        self.desc = maze_desc(self.walls, self.goal, self.collisions_stick)
 
     def initial_states(self, k: int) -> np.ndarray:
         """float64 [k, 7]: the start, heading, speed and angular velocity 0, no steps taken, no collision."""
@@ -548,10 +546,151 @@ def parse_maze(path: str):
             (float(f32(v[3])), float(f32(v[4]))), bool(flag))
 
 
+def maze_desc(walls, goal, collisions_stick) -> F.MazeDesc:
+    """The C ABI's dne_maze_desc of a parsed maze."""
+    desc = F.MazeDesc(n_walls=len(walls), collisions_stick=int(collisions_stick))
+    desc.goal[0], desc.goal[1] = goal
+    for j, w in enumerate(walls):
+        for k in range(4):
+            desc.walls[j][k] = float(w[k])
+    return desc
+
+
 def _make_maze(env_id, n_slots, seed=0, episode_len=None, maze_file=None, **kw):
     if episode_len is not None:
         raise ValueError("the maze has a fixed 400-step episode; use the episode cutoff of the config instead")
     return MazeEnv(n_slots, maze_file=maze_file, seed=seed)
+
+
+class ImageMazeEnv(BatchEnv):
+    """The hard maze seen from above as an 84x84 image (DESIGN.md 3.10), for the Atari conv policies (``LargeModelPolicy``,
+    ``GAAtariPolicy``, ``ESAtariPolicy``) under the per-tick ``dne.rollout.RolloutRunner``.  The dynamics are
+    ``MazeEnv``'s (the same device code, ``dne_image_maze_step``); a discrete action index picks a (turn, speed) row of
+    ``actions`` (default: 9 rows, each of turn and speed in {-0.5, 0, +0.5}, turn major).  Episodes are 400 steps from the
+    maze file's start; the only reward is -distance to the goal on the 400th step.  The observation is a uint8 84x84x4
+    frame stack, newest frame last, that never leaves the device: ``device_obs(lo, hi)``.  ``get_ram`` returns the final
+    (x, y), the 'final' behaviour characterisation (``bc_kind``); there is no RAM trace.  The image rule and the action
+    table are this project's definitions, not the Deep GA paper's."""
+    bc_kind = "final"
+    bc_dim = 2
+    MAX_STEPS = 400
+    DEFAULT_ACTIONS = tuple((turn, speed) for turn in (-0.5, 0.0, 0.5) for speed in (-0.5, 0.0, 0.5))
+
+    def __init__(self, n_slots: int, maze_file: Optional[str] = None, seed: int = 0, actions=None, device=None):
+        self.n_slots = int(n_slots)
+        self.maze_file = maze_file or DEFAULT_MAZE_FILE
+        self.walls, self.start, self.goal, self.collisions_stick = parse_maze(self.maze_file)
+        if len(self.walls) == 0:
+            raise ValueError(f"{self.maze_file}: the image maze needs at least one wall to frame the image")
+        tab = np.ascontiguousarray(self.DEFAULT_ACTIONS if actions is None else actions, dtype=np.float32)
+        if tab.ndim != 2 or tab.shape[1] != 2 or not 1 <= len(tab) <= F.IMAGE_MAZE_MAX_ACTIONS:
+            raise ValueError(f"actions must be [n, 2] (turn, speed) rows, 1 <= n <= {F.IMAGE_MAZE_MAX_ACTIONS}; got "
+                             f"{tab.shape}")
+        self.action_table = tab
+        self.observation_space = Box(0, 255, (84, 84, 4), dtype=np.uint8)
+        self.action_space = Discrete(len(tab))
+        self.max_episode_steps = self.MAX_STEPS
+        self.desc = maze_desc(self.walls, self.goal, self.collisions_stick)
+        self.final_xy = np.tile(np.array(self.start, dtype=np.float64), (self.n_slots, 1))
+        self.pending = np.zeros(self.n_slots, dtype=bool)      # reset, first frame not yet rendered
+        if device is None and torch.cuda.is_available():
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.device = device
+        self._b = None
+
+    def initial_states(self, k: int) -> np.ndarray:
+        """float64 [k, 7]: ``MazeEnv.initial_states``, the start at rest."""
+        s = np.zeros((int(k), 7))
+        s[:, 0], s[:, 1] = self.start
+        return s
+
+    def _bufs(self):
+        if self._b is None:
+            if self.device is None:
+                raise F.DneError("ImageMazeEnv steps on the device: no CUDA device")
+            n, dev = self.n_slots, self.device
+            pin = lambda t: t.pin_memory()                                    # noqa: E731
+            b = dict(background=torch.empty(84, 84, dtype=torch.uint8, device=dev),
+                     state=torch.zeros(n, 7, dtype=torch.float64, device=dev),
+                     stack=torch.zeros(n, 84, 84, 4, dtype=torch.uint8, device=dev),
+                     start=torch.from_numpy(self.initial_states(n)).to(dev),
+                     d_in=torch.empty(2 * n, dtype=torch.int32, device=dev),
+                     h_in=pin(torch.empty(2 * n, dtype=torch.int32)),
+                     rew=torch.empty(n, dtype=torch.float32, device=dev),
+                     done=torch.empty(n, dtype=torch.uint8, device=dev),
+                     pos=torch.empty(n, 2, dtype=torch.float64, device=dev),
+                     h_rew=pin(torch.empty(n, dtype=torch.float32)), h_done=pin(torch.empty(n, dtype=torch.uint8)),
+                     h_pos=pin(torch.empty(n, 2, dtype=torch.float64)))
+            F.check(F.lib().dne_image_maze_background(C.byref(self.desc), F.ptr(b["background"]), F.stream_ptr()))
+            self._b = b
+        return self._b
+
+    def _flush_resets(self, slots: np.ndarray) -> None:
+        """Render the first frame of the listed slots that were reset since, on the current stream."""
+        todo = slots[self.pending[slots]]
+        if len(todo) == 0:
+            return
+        b = self._bufs()
+        d_slots = torch.from_numpy(todo.astype(np.int32)).to(self.device)       # pageable: staged before the call returns
+        F.check(F.lib().dne_image_maze_reset(C.byref(self.desc), F.ptr(b["background"]), F.ptr(b["start"]),
+                                             F.ptr(d_slots), len(todo), F.ptr(b["state"]), F.ptr(b["stack"]),
+                                             F.stream_ptr()))
+        self.pending[todo] = False
+
+    def reset(self, slots):
+        """Marks the slots reset; their first frames are rendered on the stream of the next ``device_obs`` / ``step`` /
+        ``obs_block`` that covers them."""
+        slots = np.asarray(slots, dtype=np.int64)
+        self.pending[slots] = True
+        self.final_xy[slots] = self.start
+
+    def step(self, slots, actions):
+        """Steps the listed slots on the current stream (one small upload, one launch, one copy back and one sync).
+        ``actions``: indices into the action table.  Returns host (rewards float32 [k], done bool [k])."""
+        slots = np.asarray(slots, dtype=np.int64)
+        a = np.asarray(actions).astype(np.int64).reshape(-1)
+        k = len(slots)
+        if len(a) != k:
+            raise ValueError(f"{len(a)} actions for {k} slots")
+        if k == 0:
+            return np.zeros(0, np.float32), np.zeros(0, bool)
+        if a.min() < 0 or a.max() >= len(self.action_table):
+            raise ValueError(f"action index outside 0..{len(self.action_table) - 1}")
+        self._flush_resets(slots)
+        b = self._bufs()
+        b["h_in"][:k] = torch.from_numpy(slots.astype(np.int32))
+        b["h_in"][k:2 * k] = torch.from_numpy(a.astype(np.int32))
+        b["d_in"][:2 * k].copy_(b["h_in"][:2 * k], non_blocking=True)
+        F.check(F.lib().dne_image_maze_step(
+            C.byref(self.desc), F.ptr(b["background"]), self.action_table.ctypes.data_as(C.c_void_p),
+            len(self.action_table), F.ptr(b["d_in"]), C.c_void_p(b["d_in"].data_ptr() + 4 * k), k, F.ptr(b["state"]),
+            F.ptr(b["stack"]), F.ptr(b["rew"]), F.ptr(b["done"]), F.ptr(b["pos"]), F.stream_ptr()))
+        b["h_rew"][:k].copy_(b["rew"][:k], non_blocking=True)
+        b["h_done"][:k].copy_(b["done"][:k], non_blocking=True)
+        b["h_pos"][:k].copy_(b["pos"][:k], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        self.final_xy[slots] = b["h_pos"][:k].numpy()
+        return b["h_rew"][:k].numpy().copy(), b["h_done"][:k].numpy().astype(bool)
+
+    def device_obs(self, lo: int, hi: int) -> torch.Tensor:
+        """uint8 [hi-lo, 84, 84, 4] frame stacks of slots [lo, hi), ready on the current CUDA stream (a view: the next
+        ``step`` of these slots rewrites it)."""
+        self._flush_resets(np.arange(lo, hi))
+        return self._bufs()["stack"][lo:hi]
+
+    def obs_block(self, lo: int, hi: int) -> torch.Tensor:
+        """A host copy of the frame stacks of slots [lo, hi) (the virtual batch norm's reference batch)."""
+        return self.device_obs(lo, hi).cpu()
+
+    def get_ram(self, slots):
+        """float64 [k, 2]: the (x, y) after each slot's last step (the start after a reset)."""
+        return self.final_xy[np.asarray(slots, dtype=np.int64)].copy()
+
+
+def _make_image_maze(env_id, n_slots, seed=0, episode_len=None, maze_file=None, actions=None, **kw):
+    if episode_len is not None:
+        raise ValueError("the image maze has a fixed 400-step episode; use the episode cutoff of the config instead")
+    return ImageMazeEnv(n_slots, maze_file=maze_file, seed=seed, actions=actions)
 
 
 ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_len=, **kw) -> BatchEnv (real emulators plug in here)
@@ -563,4 +702,5 @@ ENV_BACKENDS = {         # id prefix -> factory(env_id, n_slots, seed=, episode_
     "MountainCar-v0": _make_mountaincar,         # MountainCarContinuous-v0 does not match this prefix
     "gym.MountainCar-v0": _make_mountaincar,
     "maze": _make_maze,                          # gym_tensorflow.make('maze', ...) of the reference GPU path
+    "ImageHardMaze-v0": _make_image_maze,        # the same maze as an 84x84 image (Such et al. 2017's Image Hard Maze)
 }

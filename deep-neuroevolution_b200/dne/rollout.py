@@ -100,6 +100,9 @@ class RolloutRunner:
         """Evaluate every unit once.  ``collect_bc``: None | 'trace' (RAM after every step, ES Atari,
         policies.py:410,418) | 'final' (RAM / position at episode end, policies.py:510,292-299)."""
         G, env = self.G, self.env
+        if collect_bc == "trace" and getattr(env, "bc_kind", "trace") != "trace":
+            raise NotImplementedError(f"{type(env).__name__} has no RAM trace: its behaviour characterisation is "
+                                      f"collect_bc={env.bc_kind!r}")
         n_units = len(units)
         limit = env.max_episode_steps if timestep_limit is None else \
             (timestep_limit if env.max_episode_steps is None else min(timestep_limit, env.max_episode_steps))

@@ -101,6 +101,14 @@ def compute_novelty_vs_archive(archive: BCArchive, bcs, k: int) -> np.ndarray:
     return nov.cpu().numpy()
 
 
+def choose_bc_mode(env, net) -> str:
+    """The behaviour characterisation ``runner.run(collect_bc=...)`` records: the environment's ``bc_kind`` when it sets
+    one (``ImageMazeEnv``: 'final', the final (x, y) behind Atari-shaped observations), otherwise per policy family: the
+    RAM trace for the Atari policies (policies.py:410,418), the final (x, y) position for MujocoPolicy
+    (policies.py:292-299, bc_choice default)."""
+    return getattr(env, "bc_kind", None) or ("final" if net.ob_kind == F.OB_VECTOR else "trace")
+
+
 def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=256, env=None, noise=None, seed=None,
                on_iteration=None):
     """nses.py:58-316."""
@@ -134,10 +142,8 @@ def run_master(master_redis_cfg, log_dir, exp, *, max_iterations=None, n_slots=2
         policy.set_ref_batch(get_ref_batch(env, batch_size=128, rs=np.random.RandomState(seed)))
     runner = make_runner(ctx, policy.net, env, n_slots=n_slots, group=2, pipeline=2 if n_slots % 4 == 0 else 1,
                          ref_batch=policy.ref_batch, **policy.runner_head_kw())
-    # behaviour characterisation per policy family: RAM trace for the Atari policies (policies.py:410,418), final (x, y)
-    # position for MujocoPolicy (policies.py:292-299, bc_choice default)
-    vector_bc = policy.net.ob_kind == F.OB_VECTOR
-    bc_mode = "final" if vector_bc else "trace"
+    bc_mode = choose_bc_mode(env, policy.net)
+    vector_bc = bc_mode == "final"
     archive = BCArchive(dev, kind="vector" if vector_bc else "trace")
     ob_stat = RunningStat(env.observation_space.shape, eps=1e-2) if policy.needs_ob_stat else None      # nses.py:72-75
     ob_count_this_batch = 0

@@ -313,6 +313,31 @@ int dne_maze_binned_episodes(dne_ctx* ctx, const dne_maze_desc* maze, const dne_
                              double* d_final_state, double* d_ob_sum, double* d_ob_sumsq, const float* bin_values_host,
                              int n_bins, int cluster, void* stream);
 
+/* The hard maze seen from above as an 84x84 uint8 image (DESIGN.md 3.10), stepped one tick at a time for the Atari conv
+ * policies.  The dynamics are dne_maze_episodes' (the same device code); the image is this project's own rendering rule:
+ * the walls' bounding box mapped uniformly onto 84x84 (aspect kept, anchored at the lower bounds, row = y), each pixel
+ * tested at its centre; 255 where a wall lies within half a pixel, 0 elsewhere; the navigator a disc of radius 8 maze
+ * units over that, 64 on its front half (towards the heading) and 128 on the back.  The goal is not drawn.
+ * Every entry takes `maze` with 1..DNE_MAZE_MAX_WALLS walls spanning a nonzero area (else DNE_ERR_ARG).
+ * dne_image_maze_background  the walls alone into d_plane uint8 [84][84]: once per maze.
+ * dne_image_maze_reset       for e < k: d_state[d_slots[e]] = d_init[e] (double[7], dne_maze_episodes' state layout),
+ *                            and all four planes of d_stacks[d_slots[e]] (uint8 [84][84][4], NHWC) set to its frame.
+ * dne_image_maze_step        for e < k: slot d_slots[e] steps with action row d_actions[e] of actions_host (the HOST
+ *                            table float32 [n_actions][2] = (turn, speed), copied into the launch; an index outside
+ *                            0..n_actions-1 steps as row 0), exactly as dne_maze_episodes steps a head output;
+ *                            d_reward[e] float32 (0, and -distance to the goal on the 400th step), d_done[e] = (t >= 400),
+ *                            d_pos[e] double[2] = the new (x, y) (nullable); the new frame is appended to the slot's
+ *                            stack as plane 3 after planes 1..3 move to 0..2.
+ * d_background is dne_image_maze_background's plane for the same maze.  The listed slots must be distinct.  Enqueued on
+ * `stream`, no host sync. */
+#define DNE_IMAGE_MAZE_MAX_ACTIONS 32
+int dne_image_maze_background(const dne_maze_desc* maze, uint8_t* d_plane, void* stream);
+int dne_image_maze_reset(const dne_maze_desc* maze, const uint8_t* d_background, const double* d_init,
+                         const int32_t* d_slots, int k, double* d_state, uint8_t* d_stacks, void* stream);
+int dne_image_maze_step(const dne_maze_desc* maze, const uint8_t* d_background, const float* actions_host, int n_actions,
+                        const int32_t* d_slots, const int32_t* d_actions, int k, double* d_state, uint8_t* d_stacks,
+                        float* d_reward, uint8_t* d_done, double* d_pos, void* stream);
+
 /* Observation statistics of the running normaliser (es.py:356-363 rollout_and_update_ob_stat; RunningStat es.py:26-48):
  * adds the observations d_obs[slot, :] (float32 [*, ob_dim], the unnormalised vectors fed to this tick's forward) of the m
  * listed slots -- the slots whose episode was sampled with probability calc_obstat_prob -- into float64 running sums

@@ -27,9 +27,9 @@
 //     into the ring stage that will hold the operand tile, NSTB chunks deep; converter warps read the raw rows from shared
 //     memory, perturb + split, and overwrite the SAME stage with the canonical [B_hi ; B_lo] tile.
 //   * persistent CTAs (one per SM), warpgroup-specialised: two MMA warpgroups (each owns every other m64 tile of the
-//     member's rows and runs the fused epilogue from its registers), one converter warpgroup, and a producer warpgroup (image
-//     TMA warp + weight TMA warp).  setmaxnreg moves registers from the converter / producer warpgroups to the MMA
-//     warpgroups, whose accumulators take 128 registers per thread.  A groups (TMA or converters <-> MMA) and the B ring
+//     member's rows and runs the fused epilogue through a shared-memory staging tile), one converter warpgroup, and a
+//     producer warpgroup (image TMA warp + weight TMA warp).  setmaxnreg moves registers from the converter / producer
+//     warpgroups to the MMA warpgroups, whose accumulators take 128 registers per thread.  A groups (TMA or converters <-> MMA) and the B ring
 //     (converters <-> MMA) run ahead of the MMA warpgroups, so staging of member i+1 overlaps the MMAs and epilogue of i.
 //   * arithmetic: wgmma kind f16 on 2 x fp16 splits (wgmma.cuh: x = h0 + h1*2^-11, 22 significand bits; uint8 pixels
 //     are exact in fp16 and need one plane) -- twice the MAC rate and half the operand bytes of a 3xTF32 formulation:
@@ -110,9 +110,14 @@ struct S2dCfg {
     static constexpr int RAW_BYTES = 2 * TPC * PIECE_STRIDE;
     static constexpr int BST_BYTES = (cmax(B_TILE, RAW_BYTES) + 127) / 128 * 128;
     static constexpr int FRAME_REGION = IN_U8 ? 2 * S2D_FRAME_STRIDE : 0;        // double-buffered raw uint8 frame
-    static constexpr int NSTB = cmin(S2D_MAX_BST, (S2D_SMEM_BUDGET - A_REGION - FRAME_REGION - 256) / BST_BYTES);
-    static_assert(NSTB >= 2, "shared memory: B ring too shallow");
-    static constexpr int SMEM_BYTES = A_REGION + NSTB * BST_BYTES + FRAME_REGION + 256;
+    // epilogue staging, one m64 tile [64][COUT] fp32 per MMA warpgroup: apart from the A region (the next member's image
+    // is loading while the epilogue runs) and from the ring
+    static constexpr int STAGE_BYTES = 64 * COUT * 4;
+    static constexpr int STAGE_REGION = 2 * STAGE_BYTES;
+    static constexpr int NSTB = cmin(S2D_MAX_BST, (S2D_SMEM_BUDGET - A_REGION - FRAME_REGION - STAGE_REGION - 256) / BST_BYTES);
+    static_assert(NSTB >= 5, "shared memory: B ring too shallow to hide a stage's TMA -> conversion -> MMA cycle");
+    static constexpr int SMEM_BYTES = A_REGION + NSTB * BST_BYTES + FRAME_REGION + STAGE_REGION + 256;
+    static_assert(SMEM_BYTES <= S2D_SMEM_BUDGET, "shared memory budget");
     static constexpr int B_UNITS = COUT * TPC * 2;               // (column n, k octet) units per chunk
     // converter groups: chunk c is converted by group c % NGRP (independent streams hide the per-chunk hand-off latency)
     static constexpr int NGRP = 2;
@@ -133,68 +138,103 @@ struct S2dOut {
 };
 
 // ------------------------------------------------------------------------------------------------------------------
-// the pair (v0, v1) of fp32 values -> one 4-byte fp16 word of the hi plane and one of the (scaled) lo plane
-__device__ __forceinline__ void store_split_pair(uint4* p_hi, uint4* p_lo, int word, float v0, float v1) {
-    uint32_t hi, lo;
-    split_f16x2(v0, v1, hi, lo);
-    reinterpret_cast<uint32_t*>(p_hi)[word] = hi;
-    reinterpret_cast<uint32_t*>(p_lo)[word] = lo;
+// The fused epilogue of one member runs in two steps per m64 tile.  (1) registers -> shared memory: each MMA warpgroup
+// folds its accumulators (main + 2^-11 * correction) into a staging tile [64][COUT] fp32 of its own.  This is the only
+// part that has to be straight-line code (the accumulators are registers).  (2) shared memory -> global: a rolled loop
+// over (row, channel octet) of the staged tile applies (/255) + bias (+BN) + activation to eight values and writes them
+// as one 16-byte row of each fp16 split plane of the next layer's image, or as NHWC floats plus the Xc copy.  Its body is
+// the same for every tile and member, so it stays in the instruction cache: the per-register path it replaces was fetched
+// cold once per member, and that fetch set the epilogue's time.
+//
+// Octet o of staging row r sits at octet o ^ s2d_stage_swz(r): the fragment stores of a half warp (rows r .. r + 3, the
+// same octet) then hit 32 distinct banks.
+template <int COUT>
+__device__ __forceinline__ int s2d_stage_swz(int r) {
+    static_assert(COUT == 16 || COUT % 32 == 0, "staging swizzle");
+    return COUT == 16 ? (r >> 1) & 1 : r & 3;
 }
 
-// The fused epilogue of one member: registers -> (/255) + bias (+BN) + activation -> global (NHWC floats + Xc, or the next
-// layer's image).  It is straight-line code (the accumulators are registers) that runs once per member, so every
-// instruction on its path is fetched cold, and that fetch, not the stores, sets its time.  The variants keep the
-// per-value path short: MODE 0 = NHWC, 1 / 2 = next image with space-to-depth stride 1 / 2 (the divisions by the stride
-// fold away), -1 = any (read from so); FAST = no batch norm and ReLU (no branch per value).  Every variant computes each
-// value with the same operations in the same order.
-template <int COUT, int HOUT, int W, int MT, int NTW, int ACC, bool IN_U8, int MODE, bool FAST>
-__device__ __forceinline__ void s2d_epilogue(const float (&acc)[NTW][ACC], const float (&cor)[NTW][ACC], int w, int wq, int lane,
-                                             const float* sb, const float* sm, const float* si, const float* sg, const float* se,
-                                             int act, bool bn, const S2dOut& so, float* outp, int slot) {
-    constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
-    const bool next_img = MODE < 0 ? so.next_img != 0 : MODE > 0;
-    const int nS = MODE > 0 ? MODE : so.nS;
+// step (1) for tile j of this warpgroup: fragment row wq*16 + lane/4 + 8h, columns 8i + 2*(lane&3) + {0, 1}
+template <int COUT, int NTW, int ACC>
+__device__ __forceinline__ void s2d_stage_tile(const float (&acc)[NTW][ACC], const float (&cor)[NTW][ACC], int j, int wq,
+                                               int lane, uint32_t stage) {
 #pragma unroll
-    for (int j = 0; j < NTW; ++j) {
-        const int t = w + 2 * j;
-        if (t >= MT) continue;
+    for (int jj = 0; jj < NTW; ++jj) {
+        if (jj != j) continue;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            const int m = t * 64 + wq * 16 + (lane >> 2) + 8 * h;
-            const int oy = m / W, ox = m - oy * W;
-            if (oy >= HOUT || ox >= HOUT) continue;
+            const int r = wq * 16 + (lane >> 2) + 8 * h;
+            const uint32_t row = stage + (uint32_t)(r * COUT + 2 * (lane & 3)) * 4;
 #pragma unroll
             for (int i = 0; i < COUT / 8; ++i) {
-                const int n = 8 * i + 2 * (lane & 3);
-                float v[2];
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    float r = fmaf(cor[j][4 * i + 2 * h + e], F16_LO_INV, acc[j][4 * i + 2 * h + e]);   // main + 2^-11 * correction
-                    if (IN_U8) r *= IN_SCALE;
-                    r += sb[n + e];
-                    if (FAST) {
-                        v[e] = fmaxf(r, 0.0f);
-                    } else {
-                        if (bn) r = (r - sm[n + e]) * si[n + e] * sg[n + e] + se[n + e];   // policies.py:322
-                        v[e] = act == DNE_ACT_RELU ? fmaxf(r, 0.0f) : (act == DNE_ACT_TANH ? tanhf(r) : r);
-                    }
-                }
-                if (!next_img) {
-                    *reinterpret_cast<float2*>(outp + (int64_t)(oy * HOUT + ox) * COUT + n) = make_float2(v[0], v[1]);
-                    if (so.xc) {
-                        const int ko = ((oy * HOUT + ox) * COUT + 8 * i) >> 3;
-                        uint4* xp = reinterpret_cast<uint4*>(so.xc) + ((int64_t)(slot >> 7) * so.xc_ko + ko) * 256 + (slot & 127);
-                        store_split_pair(xp, xp + 128, lane & 3, v[0], v[1]);
-                    }
-                } else {
-                    const int Y = oy + so.nPADB, X = ox + so.nPADB;
-                    const int pix = (Y / nS) * so.nW + (X / nS);
-                    const int pp = (Y % nS) * nS + (X % nS);
-                    const int co = pp * (COUT / 8) + i;                             // channel octet of the next image
-                    uint4* p = reinterpret_cast<uint4*>(outp) + (size_t)((co >> 1) * 4 + (co & 1)) * so.nPIXP + pix;
-                    store_split_pair(p, p + (size_t)2 * so.nPIXP, lane & 3, v[0], v[1]);
-                }
+                const int k = 4 * i + 2 * h;
+                const float v0 = fmaf(cor[jj][k], F16_LO_INV, acc[jj][k]);
+                const float v1 = fmaf(cor[jj][k + 1], F16_LO_INV, acc[jj][k + 1]);
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(row + (uint32_t)((i ^ s2d_stage_swz<COUT>(r)) * 32)),
+                             "f"(v0), "f"(v1) : "memory");
             }
+        }
+    }
+}
+
+// step (2) for tile t: thread k of the warpgroup takes row k % 64 and the octets k / 64, k / 64 + 2, ...
+template <int COUT, int HOUT, int W, bool IN_U8>
+__device__ __forceinline__ void s2d_store_tile(int t, int k, uint32_t stage, const float* sb, const float* sm, const float* si,
+                                               const float* sg, const float* se, int act, bool bn, const S2dOut& so,
+                                               float* outp, int slot) {
+    constexpr float IN_SCALE = IN_U8 ? (1.0f / 255.0f) : 1.0f;
+    constexpr int NO = COUT / 8;
+    const int ri = k & 63, m = t * 64 + ri;
+    const int oy = m / W, ox = m - oy * W;
+    if (oy >= HOUT || ox >= HOUT) return;                        // junk accumulator row
+    const uint32_t row = stage + (uint32_t)(ri * COUT) * 4;
+    const int swz = s2d_stage_swz<COUT>(ri);
+    // the fp16 split rows of octet 0: the next image's pixel (hi plane, lo plane 2 * nPIXP further) or the Xc row pair
+    uint4* p_hi = nullptr;
+    int lo_off = 0, step = 0;                                    // step: uint4 between the rows of consecutive octets
+    if (so.next_img) {
+        const int Y = oy + so.nPADB, X = ox + so.nPADB;
+        const int pix = (Y / so.nS) * so.nW + (X / so.nS);
+        const int pp = (Y % so.nS) * so.nS + (X % so.nS);        // channel octets pp * NO .. of the next image
+        p_hi = reinterpret_cast<uint4*>(outp) + (int64_t)pp * (NO / 2) * 4 * so.nPIXP + pix;
+        lo_off = 2 * so.nPIXP;
+        step = so.nPIXP;
+    } else if (so.xc) {
+        p_hi = reinterpret_cast<uint4*>(so.xc) + ((int64_t)(slot >> 7) * so.xc_ko + (oy * HOUT + ox) * NO) * 256 + (slot & 127);
+        lo_off = 128;
+        step = 256;
+    }
+#pragma unroll 1
+    for (int o = k >> 6; o < NO; o += 2) {
+        float v[8];
+        {
+            float4 x0, x1;
+            const uint32_t a = row + (uint32_t)((o ^ swz) * 32);
+            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x0.x), "=f"(x0.y), "=f"(x0.z), "=f"(x0.w) : "r"(a));
+            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x1.x), "=f"(x1.y), "=f"(x1.z), "=f"(x1.w) : "r"(a + 16));
+            v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const int n = 8 * o + e;
+            float r = v[e];
+            if (IN_U8) r *= IN_SCALE;
+            r += sb[n];
+            if (bn) r = (r - sm[n]) * si[n] * sg[n] + se[n];   // policies.py:322
+            v[e] = act == DNE_ACT_RELU ? fmaxf(r, 0.0f) : (act == DNE_ACT_TANH ? tanhf(r) : r);
+        }
+        if (!so.next_img) {
+            float4* dst = reinterpret_cast<float4*>(outp + (int64_t)(oy * HOUT + ox) * COUT + 8 * o);
+            dst[0] = make_float4(v[0], v[1], v[2], v[3]);
+            dst[1] = make_float4(v[4], v[5], v[6], v[7]);
+        }
+        if (p_hi) {
+            // next image: octet pp * NO + o is plane (o & 1) of plane pair (pp * NO + o) / 2 (NO is even)
+            const int po = so.next_img ? ((o >> 1) * 4 + (o & 1)) * step : o * step;
+            uint4 hi, lo;
+            split_f16x8(v, hi, lo);
+            p_hi[po] = hi;
+            p_hi[po + lo_off] = lo;
         }
     }
 }
@@ -222,6 +262,7 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
     const uint32_t sA = smem_u32(smem), sB = sA + Cfg::A_REGION;
     uint8_t* const gB = smem + Cfg::A_REGION;                                    // generic view of the ring (bulk copies)
     uint8_t* const gFrame = gB + NSTB * Cfg::BST_BYTES;
+    uint8_t* const gStage = gFrame + Cfg::FRAME_REGION;                         // epilogue staging of the MMA warpgroups
 
     if (tid == 0) {
         for (int i = 0; i < NG; ++i) {
@@ -323,22 +364,21 @@ conv_s2d_kernel(SlotArgs sa, int64_t off_w, LayerEpi epi, const void* __restrict
             }
             mbar_arrive(&b_empty[(cb - 1) % NSTB]);
             mbar_arrive(&a_empty[NG - 1]);
-            named_bar_sync(2, S2D_MMA_THREADS);                  // per-channel parameters (and padding) of this member ready
-            // ---- epilogue: registers -> (/255) + bias (+BN) + activation -> global ----
+            named_bar_sync(2, S2D_MMA_THREADS);                  // per-channel parameters (and padding) of this member ready,
+                                                                 // and the staging tiles of the previous member read
+            // ---- epilogue, one tile at a time: registers -> staging tile -> (/255) + bias (+BN) + activation -> global ----
             {
                 const float *sb = s_bias[pb], *sm = s_mean[pb], *si = s_inv[pb], *sg = s_gamma[pb], *se = s_beta[pb];
-                const bool relu_only = !bn && act == DNE_ACT_RELU;
-#define S2D_EPI(MODE, FAST)                                                                                              \
-    s2d_epilogue<COUT, HOUT, W, MT, NTW, Cfg::ACC, IN_U8, MODE, FAST>(acc, cor, w, wq, lane, sb, sm, si, sg, se, act, bn, so, \
-                                                                       outp, slot)
-                // the fast variant writes what follows this shape in the compiled nets (the shape list below): 32 -> 64
-                // channels -> a stride-1 image, the others -> NHWC.  The first layer keeps the generic one: its 128
-                // accumulator registers leave no room for a second copy (ptxas spills them).
-                constexpr int FAST_MODE = CIN == 32 ? 1 : 0;
-                if (!IN_U8 && relu_only && (FAST_MODE == 0 ? !so.next_img : (so.next_img && so.nS == FAST_MODE)))
-                    S2D_EPI(FAST_MODE, true);
-                else S2D_EPI(-1, false);
-#undef S2D_EPI
+                const uint32_t stage = smem_u32(gStage) + w * Cfg::STAGE_BYTES;
+#pragma unroll 1
+                for (int j = 0; j < NTW; ++j) {
+                    const int t = w + 2 * j;
+                    if (t >= MT) break;                          // warpgroup-uniform
+                    if (j > 0) named_bar_sync(5 + w, 128);       // the previous tile is read
+                    s2d_stage_tile<COUT, NTW, Cfg::ACC>(acc, cor, j, wq, lane, stage);
+                    named_bar_sync(5 + w, 128);
+                    s2d_store_tile<COUT, HOUT, W, IN_U8>(t, tid & 127, stage, sb, sm, si, sg, se, act, bn, so, outp, slot);
+                }
             }
             ++it;
         }
